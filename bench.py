@@ -91,7 +91,7 @@ def synth_workload(cfg, image=0):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -137,24 +137,22 @@ class ClockSampler:
 
 
 def peaks():
+    """(HBM GB/s, dense fp16 TFLOP/s, sustained dense fp16 TFLOP/s, source). Without MEASURED_PEAKS.json: the H100 SXM
+    data sheet (3.35 TB/s, 989 TFLOP/s dense at up to 700 W), which is not a rate the card was measured to reach."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "fallback"
 
 
-def ncu_traffic(kernel_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture of this
-    round (profiles/r02_ncu_traffic.json, written from the .ncu-rep by tools/ncu_traffic.py), or None."""
-    p = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    if not os.path.exists(p):
-        return None, None
-    with open(p) as f:
-        d = json.load(f)
-    e = d.get(kernel_key)
-    return (e["bytes_per_launch"], e["note"]) if e else (None, None)
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: the arrays the timed path computed in its last step, one float32 DIR/<name>.npy each."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def host_threads():
@@ -390,6 +388,14 @@ def run_product_xl(args, rank, world, local_rank):
         ms = e0.elapsed_time(e1)
         launches = ops.LAUNCHES - launches0
         clk = clocks.stop() if clocks else None
+    if args.dump_outputs:
+        # the latents each image's last timed rich_text_step produced (+ its colour loss); one writer per image
+        rpi = image_groups(world, rank, cfg["images"])[1] if cfg["images"] > 1 else world
+        if rank % rpi == 0:
+            arrays = {f"latents_image{im}": st.latents for im, st in zip(my_images, states)}
+            if cfg["color"] and "color_loss" in model.last_step_stats:
+                arrays[f"color_loss_image{my_images[-1]}"] = model.last_step_stats["color_loss"].reshape(-1)
+            dump_outputs(args.dump_outputs, arrays)
     t = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -519,8 +525,8 @@ def run_product_xl(args, rank, world, local_rank):
         n_prof = len(prof_idx)
         if s:
             ach = s[1] / s[0] / 1e12
-            traffic, tnote = ncu_traffic("attn_self_kernel")
-            roof = {"kernel": "attn_self_kernel<NV> (self-attention, tcgen05/TMEM/TMA, head_dim 64, grouped PV on injection steps)",
+            traffic, tnote = None, "not measured"
+            roof = {"kernel": "attn_fwd_kernel (self-attention, wgmma/TMA, head_dim 64, 64-key tiles)",
                     "bound": "tensor", "achieved": ach, "peak": tf_sust, "unit": "TFLOP/s", "frac": ach / tf_sust,
                     "flops_counted": "algorithmic: QK^T once per score source + PV per entry (what the reference evaluates)",
                     "traffic": traffic, "traffic_note": tnote,
@@ -528,8 +534,8 @@ def run_product_xl(args, rank, world, local_rank):
                     "launches_timed": s[3], "profiled_steps": n_prof, "ms_per_step_in_kernel": s[0] * 1e3 / n_prof}
         if c:
             gbs = c[2] / c[0] / 1e9
-            ctraffic, cnote = ncu_traffic("attn_fwd_kernel_cross")
-            cross = {"kernel": "attn_cross_kernel (cross-attention, 77 keys, font-size re-weighting on pass B; persistent, TMA ring + tcgen05/TMEM)", "bound": "hbm", "achieved": gbs,
+            ctraffic, cnote = None, "not measured"
+            cross = {"kernel": "attn_fwd_kernel (cross-attention, 77 keys, font-size re-weighting on pass B; wgmma/TMA)", "bound": "hbm", "achieved": gbs,
                      "peak": hbm, "unit": "GB/s", "frac": gbs / hbm, "tensor_tflops": c[1] / c[0] / 1e12,
                      "traffic": ctraffic, "traffic_note": cnote,
                      "launches_timed": c[3], "ms_per_step_in_kernel": c[0] * 1e3 / n_prof}
@@ -655,6 +661,8 @@ def run_product_sd(args, rank, world, local_rank):
         launches = ops.LAUNCHES - launches0
         clk = clocks.stop() if clocks else None
         assert bool(torch.isfinite(out.float()).all())
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"latents": out})
         host_lat = torch.empty(1, 4, 64, 64, dtype=torch.float16).pin_memory()
         barrier()
         t0 = time.perf_counter()
@@ -712,6 +720,8 @@ def main():
     ap.add_argument("--impl", default="rtti", choices=["rtti", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--check", action="store_true", help="N > 1: also compare with a single-GPU run of the same steps")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what their last step computed to DIR/<name>.npy (float32)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,4 +1,4 @@
-/* rtti_b200 — C ABI of the B200-native region-diffusion hot path.
+/* rtti_b200 — C ABI of the region-diffusion hot path for the H100 (sm_90a).
  *
  * The reference (songweige/rich-text-to-image) has no FFI: its hot path is Python calling ATen.
  * Each entry point below replaces one (group of) reference call site(s); citations are
@@ -11,7 +11,7 @@
  *     (a cudaStream_t passed as void*); all are CUDA-graph capturable.
  *   - fp16 = IEEE binary16 (`__half`), row-major, innermost dimension contiguous.
  *   - Return value: RTTI_OK (0) or a negative RTTI_ERR_* code; nothing is launched on error.
- *   - The caller selects the device (cudaSetDevice) before the call; sm_100 is required.
+ *   - The caller selects the device (cudaSetDevice) before the call; sm_90 is required.
  */
 #ifndef RTTI_B200_H
 #define RTTI_B200_H
@@ -24,7 +24,7 @@ extern "C" {
 #define RTTI_ERR_ARG (-1)    /* null pointer / out-of-range argument */
 #define RTTI_ERR_SHAPE (-2)  /* unsupported shape (e.g. head_dim not a multiple of 8 or > 192) */
 #define RTTI_ERR_ALIGN (-3)  /* pointer not 16-byte aligned / stride not a multiple of 8 elements */
-#define RTTI_ERR_ARCH (-4)   /* device is not sm_100 */
+#define RTTI_ERR_ARCH (-4)   /* device is not sm_90 */
 #define RTTI_ERR_CUDA (-5)   /* CUDA runtime / driver call failed (see cudaGetLastError) */
 
 /* Library version: major*10000 + minor*100 + patch. */
@@ -32,7 +32,7 @@ int rtti_version(void);
 /* RTTI_OK when the current device can run these kernels (compute capability 10.x). */
 int rtti_arch_ok(void);
 
-/* Fused attention forward: O = softmax(scale * Q K^T) V per head, on tcgen05 tensor cores.
+/* Fused attention forward: O = softmax(scale * Q K^T) V per head, on wgmma tensor cores.
  * Replaces Attention.get_attention_scores + torch.bmm + reshape_batch_dim_to_heads_and_average
  * (models/attention_processor.py:359-407, 1157-1163, 166-171, 1181) and the hook passes that
  * sit around them (models/region_diffusion_sdxl.py:959-1140).
@@ -91,7 +91,7 @@ int rtti_add_bias_f16(const void* a, const void* b, const void* bias, void* out,
 int rtti_layernorm_fwd(const void* x, const void* gamma, const void* beta, void* y, int rows, int c, float eps,
                        void* stream);
 
-/* Feed-forward input projection with the GEGLU gate fused into the GEMM epilogue (tcgen05 GEMM, TMEM accumulators):
+/* Feed-forward input projection with the GEGLU gate fused into the GEMM epilogue (wgmma GEMM, register accumulators):
  *   y[m, n] = (x[m, k] w[0:n, :]^T + bias[0:n]) * gelu(x w[n:2n, :]^T + bias[n:2n])     (exact erf GELU)
  * x [m, k], w [2n, k] (the nn.Linear weight of ff.net.0.proj: value rows first, gate rows second), y [m, n], all fp16
  * row-major contiguous; bias [2n] fp16 or NULL. Replaces models/attention.py:283-304 (GEGLU.forward: proj -> chunk ->

@@ -323,10 +323,90 @@ def gen_token_maps(ns):
     print("token maps ok", [float(x.mean()) for x in masks])
 
 
+def to_json(x):
+    """JSON form of a reference result: tensors (with dtype), tuples and dicts kept distinguishable."""
+    if torch.is_tensor(x):
+        return {"__tensor__": x.detach().cpu().tolist(), "dtype": str(x.dtype).replace("torch.", "")}
+    if isinstance(x, tuple):
+        return {"__tuple__": [to_json(v) for v in x]}
+    if isinstance(x, list):
+        return [to_json(v) for v in x]
+    if isinstance(x, dict):
+        return {"__dict__": [[to_json(k), to_json(v)] for k, v in x.items()]}
+    return x
+
+
+def from_json(x):
+    if isinstance(x, dict):
+        if "__tensor__" in x:
+            return torch.tensor(x["__tensor__"], dtype=getattr(torch, x["dtype"]))
+        if "__tuple__" in x:
+            return tuple(from_json(v) for v in x["__tuple__"])
+        return {from_json(k): from_json(v) for k, v in x["__dict__"]}
+    if isinstance(x, list):
+        return [from_json(v) for v in x]
+    return x
+
+
+def gen_reference_checks(ns):
+    """What tests/test_oracle_vs_reference.py compares the oracle against, taken from the unmodified reference:
+    reference_checks.npz (UNet outputs, parameter inventories, one attention call, two rich-text XL loops) and
+    richtext_reference.json (the reference's rich-text parsing functions on the test's Quill deltas)."""
+    import json
+    from tests import test_oracle_vs_reference as t
+    from tests import synth
+    res = {}
+    for name, cfg_fn, seed in (("tiny_sd", uo.tiny_sd_config, 3), ("tiny_xl", uo.tiny_xl_config, 4)):
+        cfg = cfg_fn()
+        model = ns.unet_2d_condition.UNet2DConditionModel(**cfg.ref_kwargs())
+        model.load_state_dict(uo.make_state_dict(cfg, seed))
+        x, ctx, added = t.unet_inputs(cfg, seed)
+        with torch.no_grad():
+            for i, tt in enumerate(t.UNET_TIMESTEPS):
+                res[f"unet_{name}_t{i}"] = model(x, tt, encoder_hidden_states=ctx, added_cond_kwargs=added)["sample"].numpy()
+    for name, cfg in (("sd15", uo.sd15_config()), ("sdxl", uo.sdxl_config())):
+        with torch.device("meta"):
+            model = ns.unet_2d_condition.UNet2DConditionModel(**cfg.ref_kwargs())
+        sd = model.state_dict()
+        res[f"inv_{name}_names"] = np.array(list(sd))
+        res[f"inv_{name}_shapes"] = np.array([list(v.shape) + [-1] * (4 - v.dim()) for v in sd.values()], dtype=np.int64)
+    torch.manual_seed(0)
+    attn = ns.attention_processor.Attention(query_dim=64, cross_attention_dim=48, heads=2, dim_head=32)
+    hs, ctx = torch.randn(1, 32, 64), torch.randn(1, 77, 48)
+    with torch.no_grad():
+        o, (pavg, pr) = attn(hs, None, t.attention_weights(), encoder_hidden_states=ctx)
+    res.update({"attn_hs": hs.numpy(), "attn_ctx": ctx.numpy(), "attn_out": o.numpy(), "attn_pavg": pavg.numpy(),
+                "attn_p": pr.numpy()})
+    res.update({f"attn_w_{k}": v.numpy() for k, v in attn.state_dict().items()})
+    for i, case in enumerate(t.XL_LIVE_CASES):
+        res[f"xl_live_{i}"] = t.xl_reference_loop(ns, *case).numpy().astype(np.float32)
+    np.savez_compressed(os.path.join(GOLD, "reference_checks.npz"), **res)
+    rr = ns.richtext_utils
+    out = []
+    for delta in t._DELTAS:
+        parsed = rr.parse_json(delta)
+        base, styles, notes, note_t, cspans, cnames, crgbs, sizes, use_grad = parsed
+        region = rr.get_region_diffusion_input(t._Model(), base, styles, notes, note_t, cspans, cnames)
+        ctrl = rr.get_attention_control_input(t._Model(), region[2], sizes)
+        grad = rr.get_gradient_guidance_input(t._Model(), region[2], cspans, crgbs, dict(ctrl), color_guidance_weight=0.5)
+        rec = {"parse_json": parsed, "region": region, "control": ctrl, "gradient": grad}
+        back = from_json(json.loads(json.dumps(to_json(rec))))
+        for k in rec:
+            a, b = rec[k], back[k]
+            if isinstance(a, dict):
+                assert set(a) == set(b) and all(t.same(a[j], b[j]) for j in a)
+            else:
+                assert t.same(a, b) if k != "gradient" else (t.same(a[1], b[1]) and set(a[0]) == set(b[0]))
+        out.append(to_json(rec))
+    with open(os.path.join(GOLD, "richtext_reference.json"), "w") as f:
+        json.dump(out, f)
+    print("reference checks ok")
+
+
 def main():
     os.makedirs(GOLD, exist_ok=True)
     ns = ref_shim.import_reference()
-    which = sys.argv[1:] or ["unet", "attention", "token_maps", "sd", "xl", "xl_labels"]
+    which = sys.argv[1:] or ["unet", "attention", "token_maps", "sd", "xl", "xl_labels", "reference_checks"]
     torch.set_num_threads(max(1, os.cpu_count() or 1))
     if "unet" in which: gen_unet(ns)
     if "attention" in which: gen_attention(ns)
@@ -334,6 +414,7 @@ def main():
     if "sd" in which: gen_sd_loops(ns)
     if "xl" in which: gen_xl_loops(ns)
     if "xl_labels" in which: gen_xl_labels(ns)
+    if "reference_checks" in which: gen_reference_checks(ns)
 
 
 if __name__ == "__main__":

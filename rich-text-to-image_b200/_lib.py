@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI declared in include/rtti_b200.h.
 
 The product path has no CPU or PyTorch fallback: if the library is missing or the device is not
-sm_100 every op raises.
+sm_90 every op raises.
 """
 import ctypes
 import os
@@ -14,7 +14,7 @@ _ERRORS = {
     -1: "RTTI_ERR_ARG (null pointer / out-of-range argument)",
     -2: "RTTI_ERR_SHAPE (unsupported shape)",
     -3: "RTTI_ERR_ALIGN (pointer or stride alignment)",
-    -4: "RTTI_ERR_ARCH (device is not sm_100)",
+    -4: "RTTI_ERR_ARCH (device is not sm_90)",
     -5: "RTTI_ERR_CUDA (CUDA runtime/driver error)",
 }
 

@@ -1,23 +1,22 @@
-// Self-attention token-map capture for sm_100a: accum[q, k] += mean_h softmax(scale Q_h K_h^T)[q, k].
+// Self-attention token-map capture for sm_90a: accum[q, k] += mean_h softmax(scale Q_h K_h^T)[q, k].
 //
 // The reference materialises the full probability tensor of every attention call and averages it
 // over heads on every call (models/attention_processor.py:1157-1159, 166-171, 1181), then the
 // token-map hook copies the conditional row to the CPU and sums it there
 // (models/region_diffusion_sdxl.py:986-992). Here the flash kernel (attn_fwd.cu) leaves only the
-// per-row log-sum-exp; this kernel recomputes the 128x128 score tiles on tcgen05 tensor cores,
+// per-row log-sum-exp; this kernel recomputes the 128x128 score tiles with wgmma,
 // loops over the heads inside the CTA (so the head mean needs no atomics and is deterministic) and
 // adds the tile into an fp32 accumulator that stays on the device.
 //
-// CTA = one (128 query rows) x (128 keys) tile, all heads. Warps 0-3: exp + accumulate (thread = row =
-// TMEM lane); warp 4: TMA producer; warp 5: MMA issuer. S is double-buffered in TMEM so the MMA of
-// head h+1 overlaps the exponentials of head h.
+// CTA = one (128 query rows) x (128 keys) tile, all heads; two warpgroups of 64 rows. Thread 0 keeps the
+// Q and K tiles of the next head in flight in a two-stage TMA ring.
 #include "ptx.cuh"
 #include "rtti_internal.h"
 
 namespace rtti {
 
 struct ProbsMeanParams {
-  int heads, head_dim, n_q, n_k, ksteps_qk;
+  int heads, head_dim, n_q, n_k;
   float scale_log2, inv_heads;
   const float* lse;  // [heads, n_q]
   float* accum;      // [n_q, n_k]
@@ -25,126 +24,88 @@ struct ProbsMeanParams {
 
 template <int NDCH>
 struct PMCfg {
-  static constexpr int NSTAGE = (NDCH == 3) ? 1 : 2;
   static constexpr int TILE = 128 * 128;
-  static constexpr int OFF_Q = 0;
-  static constexpr int OFF_K = NSTAGE * NDCH * TILE;
-  static constexpr int OFF_BAR = 2 * NSTAGE * NDCH * TILE;
-  static constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
+  static constexpr int STAGE = 2 * NDCH * TILE;   // Q chunks, then K chunks
+  static constexpr int OFF_BAR = 2 * STAGE;
+  static constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;
 };
 
 template <int NDCH>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(256, 1)
 attn_probs_mean_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-                       const ProbsMeanParams p) {
+                       const __grid_constant__ ProbsMeanParams p) {
   using C = PMCfg<NDCH>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-  uint64_t* full = bars;         // [NSTAGE] TMA -> MMA
-  uint64_t* empty = bars + 2;    // [NSTAGE] MMA -> TMA
-  uint64_t* s_full = bars + 4;   // [2] MMA -> exp warps
-  uint64_t* s_empty = bars + 6;  // [2] exp warps -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);   // [2]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31;
   const int k0 = blockIdx.x * 128, q0 = blockIdx.y * 128;
 
-  if (warp == 4 && lane == 0) {
+  auto load = [&](int h) {   // thread 0
+    const int s = h & 1;
+    uint8_t* st = smem + s * C::STAGE;
+    mbar_expect_tx(&full[s], C::STAGE);
+#pragma unroll
+    for (int c = 0; c < NDCH; ++c) {
+      tma_load_4d(st + c * C::TILE, &tm_q, &full[s], 64 * c, h, q0, 0);
+      tma_load_4d(st + (NDCH + c) * C::TILE, &tm_k, &full[s], 64 * c, h, k0, 0);
+    }
+  };
+  if (tid == 0) {
     tma_prefetch_desc(&tm_q); tma_prefetch_desc(&tm_k);
-    for (int i = 0; i < C::NSTAGE; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], 128); }
+    mbar_init(&full[0], 1); mbar_init(&full[1], 1);
     mbar_fence_init();
+    load(0);
+    if (p.heads > 1) load(1);
   }
-  if (warp == 5) tmem_alloc<256>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp == 4) {
-    if (lane == 0) {
-      for (int h = 0; h < p.heads; ++h) {
-        const int st = h % C::NSTAGE;
-        mbar_wait(&empty[st], ((h / C::NSTAGE) & 1) ^ 1);
-        mbar_expect_tx(&full[st], 2 * NDCH * C::TILE);
+  const int r0 = 64 * wg + 16 * w + (lane >> 2), r1 = r0 + 8;
+  const int cq = 2 * (lane & 3);
+  const bool ok0 = q0 + r0 < p.n_q, ok1 = q0 + r1 < p.n_q;
+  const uint32_t sbase = smem_u32(smem);
+  float acc[64];
 #pragma unroll
-        for (int c = 0; c < NDCH; ++c) {
-          tma_load_4d(smem + C::OFF_Q + (st * NDCH + c) * C::TILE, &tm_q, &full[st], 64 * c, h, q0, 0);
-          tma_load_4d(smem + C::OFF_K + (st * NDCH + c) * C::TILE, &tm_k, &full[st], 64 * c, h, k0, 0);
-        }
-      }
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+  for (int h = 0; h < p.heads; ++h) {
+    const int s = h & 1;
+    const float nl0 = ok0 ? -p.lse[static_cast<size_t>(h) * p.n_q + q0 + r0] : 0.f;
+    const float nl1 = ok1 ? -p.lse[static_cast<size_t>(h) * p.n_q + q0 + r1] : 0.f;
+    const uint32_t qa = sbase + s * C::STAGE + wg * 64 * 128;
+    const uint32_t ka = sbase + s * C::STAGE + NDCH * C::TILE;
+    mbar_wait(&full[s], (h >> 1) & 1);
+    float sc[64];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4 * NDCH; ++kk) {
+      const uint32_t off = (kk >> 2) * C::TILE + (kk & 3) * 32;
+      wgmma_ss<128>(sc, wgmma_desc_sw128(qa + off, 16, 1024), wgmma_desc_sw128(ka + off, 16, 1024), kk > 0 ? 1u : 0u);
     }
-  } else if (warp == 5) {
-    if (lane == 0) {
-      constexpr uint32_t IDESC = umma_idesc_f16(128, 128, 0, 0);
-      const uint32_t smem_base = smem_u32(smem);
-      for (int h = 0; h < p.heads; ++h) {
-        const int st = h % C::NSTAGE, sb = h & 1;
-        mbar_wait(&full[st], (h / C::NSTAGE) & 1);
-        mbar_wait(&s_empty[sb], ((h >> 1) & 1) ^ 1);
-        tc_fence_after();
-        for (int kk = 0; kk < p.ksteps_qk; ++kk) {
-          const int c = kk >> 2, k16 = kk & 3;
-          const uint64_t da = umma_desc_sw128(smem_base + C::OFF_Q + (st * NDCH + c) * C::TILE + k16 * 32, 0, 1024);
-          const uint64_t db = umma_desc_sw128(smem_base + C::OFF_K + (st * NDCH + c) * C::TILE + k16 * 32, 0, 1024);
-          mma_f16_ss(tmem + 128 * sb, da, db, IDESC, kk > 0);
-        }
-        tc_commit(&empty[st]);
-        tc_commit(&s_full[sb]);
-      }
-    }
-  } else {
-    const int row = warp * 32 + lane;
-    const uint32_t tlane = tmem + (static_cast<uint32_t>(warp * 32) << 16);
-    const bool row_ok = (q0 + row) < p.n_q;
-    float acc[128];
+    wgmma_commit();
+    wgmma_wait_all<64>(sc);
+    __syncthreads();   // both warpgroups are done with stage s
+    if (tid == 0 && h + 2 < p.heads) load(h + 2);
 #pragma unroll
-    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-    for (int h = 0; h < p.heads; ++h) {
-      const int sb = h & 1;
-      const float neg_lse = row_ok ? -p.lse[static_cast<size_t>(h) * p.n_q + q0 + row] : 0.f;
-      mbar_wait(&s_full[sb], (h >> 1) & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t s[32];
-        tmem_ld32(tlane + 128 * sb + 32 * c, s);
-        tmem_wait_ld_regs32(s);
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float e0 = ex2_approx(fmaf(__uint_as_float(s[2 * i]), p.scale_log2, neg_lse));
-          const float e1 = ex2_approx(fmaf(__uint_as_float(s[2 * i + 1]), p.scale_log2, neg_lse));
-          // the reference averages fp16 probabilities (attention_processor.py:405, 1181)
-          const float2 r = __half22float2(__floats2half2_rn(e0, e1));
-          acc[32 * c + 2 * i] += r.x;
-          acc[32 * c + 2 * i + 1] += r.y;
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(&s_empty[sb]);
-    }
-    if (row_ok) {
-      float* dst = p.accum + static_cast<size_t>(q0 + row) * p.n_k + k0;
-      const int ncol = min(128, p.n_k - k0);
-      if (ncol == 128 && (p.n_k & 3) == 0) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float4 v = *reinterpret_cast<float4*>(dst + 4 * i);
-          v.x += acc[4 * i] * p.inv_heads; v.y += acc[4 * i + 1] * p.inv_heads;
-          v.z += acc[4 * i + 2] * p.inv_heads; v.w += acc[4 * i + 3] * p.inv_heads;
-          *reinterpret_cast<float4*>(dst + 4 * i) = v;
-        }
-      } else {
-#pragma unroll
-        for (int i = 0; i < 128; ++i)
-          if (i < ncol) dst[i] += acc[i] * p.inv_heads;
-      }
+    for (int i = 0; i < 16; ++i) {
+      // the reference averages fp16 probabilities (attention_processor.py:405, 1181)
+      const float2 a = __half22float2(__floats2half2_rn(ex2_approx(fmaf(sc[4 * i], p.scale_log2, nl0)),
+                                                        ex2_approx(fmaf(sc[4 * i + 1], p.scale_log2, nl0))));
+      const float2 c = __half22float2(__floats2half2_rn(ex2_approx(fmaf(sc[4 * i + 2], p.scale_log2, nl1)),
+                                                        ex2_approx(fmaf(sc[4 * i + 3], p.scale_log2, nl1))));
+      acc[4 * i] += a.x; acc[4 * i + 1] += a.y; acc[4 * i + 2] += c.x; acc[4 * i + 3] += c.y;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc<256>(tmem);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    if (!(r ? ok1 : ok0)) continue;
+    float* dst = p.accum + static_cast<size_t>(q0 + (r ? r1 : r0)) * p.n_k + k0;
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (k0 + 8 * i + cq + j < p.n_k) dst[8 * i + cq + j] += acc[4 * i + 2 * r + j] * p.inv_heads;
+  }
 }
 
 template <int NDCH>
@@ -152,13 +113,10 @@ static int launch_pm(const CUtensorMap& tq, const CUtensorMap& tk, const ProbsMe
                      cudaStream_t stream) {
   using C = PMCfg<NDCH>;
   auto kern = attn_probs_mean_kernel<NDCH>;
-  static bool configured = false;
-  if (!configured) {
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) != cudaSuccess)
-      return RTTI_ERR_CUDA;
-    configured = true;
-  }
-  kern<<<grid, 192, C::SMEM_BYTES, stream>>>(tq, tk, p);
+  static const bool configured =
+      cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) == cudaSuccess;
+  if (!configured) return RTTI_ERR_CUDA;
+  kern<<<grid, 256, C::SMEM_BYTES, stream>>>(tq, tk, p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }
 
@@ -178,7 +136,6 @@ extern "C" int rtti_attn_probs_mean_accum(const void* q, const void* k, const fl
   if (rc != RTTI_OK) return rc;
   ProbsMeanParams p{};
   p.heads = heads; p.head_dim = head_dim; p.n_q = n_q; p.n_k = n_k;
-  p.ksteps_qk = (head_dim + 15) / 16;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.inv_heads = 1.f / (float)heads;
   p.lse = lse; p.accum = accum;

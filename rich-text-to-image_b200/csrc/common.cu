@@ -10,7 +10,7 @@ extern "C" int rtti_arch_ok(void) {
   if (cudaGetDevice(&dev) != cudaSuccess) return RTTI_ERR_CUDA;
   int major = 0;
   if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess) return RTTI_ERR_CUDA;
-  return major == 10 ? RTTI_OK : RTTI_ERR_ARCH;
+  return major == 9 ? RTTI_OK : RTTI_ERR_ARCH;
 }
 
 namespace rtti {

@@ -559,7 +559,7 @@ extern "C" int rtti_geglu_fwd(const void* proj, void* y, int rows, int inner, vo
   if (((uintptr_t)proj | (uintptr_t)y) & 15) return RTTI_ERR_ALIGN;
   const long long total = (long long)rows * (inner / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   geglu_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const __half*)proj, (__half*)y, rows, inner);
   return ok_or_cuda();
 }
@@ -634,7 +634,7 @@ extern "C" int rtti_add_bias_f16(const void* a, const void* b, const void* bias,
   if (((uintptr_t)a | (uintptr_t)b | (uintptr_t)out | (uintptr_t)bias) & 15) return RTTI_ERR_ALIGN;
   const long long nvec = rows * (c / 8);
   long long blocks = (nvec + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   add_bias_f16_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const __half*)a, (const __half*)b, (const __half*)bias,
                                                                      (__half*)out, nvec, c / 8);
   return ok_or_cuda();

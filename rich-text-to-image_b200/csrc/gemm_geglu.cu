@@ -1,20 +1,17 @@
-// Feed-forward input projection with the GEGLU gate fused into the GEMM epilogue (sm_100a: tcgen05 + TMEM + TMA).
+// Feed-forward input projection with the GEGLU gate fused into the GEMM epilogue (sm_90a: wgmma + TMA + mbarrier).
 //
 // Reference: models/attention.py:283-304 (GEGLU.forward): `hidden_states, gate = proj(x).chunk(2, dim=-1);
 // return hidden_states * gelu(gate)` — a [M, C] x [C, 8C] GEMM whose [M, 8C] result is written, read back, gated and
 // written again as [M, 4C]. Here the value and the gate columns of one output tile are accumulated side by side in
-// TMEM (ONE M=128, N=256 MMA per k step: B tile rows 0-127 = value weights, rows 128-255 = the matching gate weights)
-// and the epilogue computes y = (v + b_v) * gelu(g + b_g) straight out of TMEM: the [M, 8C] intermediate never exists.
+// registers (per k step two wgmma M64 N128 K16 per warpgroup: B tile rows 0-127 = value weights, rows 128-255 = the
+// matching gate weights) and the epilogue computes y = (v + b_v) * gelu(g + b_g) straight from the accumulators: the
+// [M, 8C] intermediate never exists.
 //
 //   y[M, N] = (x[M, K] W[0:N, :]^T + bias[0:N]) * gelu(x[M, K] W[N:2N, :]^T + bias[N:2N]),   exact (erf) GELU
 //
-// Persistent kernel, one CTA per SM, 10 warps:
-//   warp 0      TMA producer        (A tile 128 x 64, value and gate weight tiles 128 x 64 each, 4-stage ring, SWIZZLE_128B)
-//   warp 1      MMA issuer          (4 x tcgen05.mma M128 N256 K16 per stage; accumulators double-buffered: 2 x 256 TMEM columns)
-//   warps 2-9   epilogue            (thread = output row; two warps per TMEM lane quadrant, each owning 64 of the 128
-//                                    output columns: tcgen05.ld value + gate, bias, erf-GELU, product, fp16, swizzled
-//                                    staging tile, TMA store) — overlaps the main loop of the next tile
-// The producer and the MMA warp run warp-uniform loops with predicated issue (ptx.cuh).
+// CTA = one 128 x 128 output tile, two warpgroups of 64 rows. A 4-stage ring of {A 128 x 64, value 128 x 64, gate
+// 128 x 64} tiles (SWIZZLE_128B) is filled by TMA from thread 0, which refills a stage after the barrier that ends the
+// k block that read it.
 #include "ptx.cuh"
 #include "rtti_internal.h"
 
@@ -24,162 +21,88 @@ constexpr int BM = 128, BN = 128, BK = 64;
 constexpr int STAGES = 4;
 constexpr int A_TILE = BM * BK * 2;        // 16 KB
 constexpr int B_TILE = 2 * BN * BK * 2;    // 32 KB: value rows then gate rows
-constexpr int O_TILE = BM * 64 * 2;        // 16 KB per 64-column half
-constexpr int OFF_A = 0;
-constexpr int OFF_B = OFF_A + STAGES * A_TILE;
-constexpr int OFF_O = OFF_B + STAGES * B_TILE;
-constexpr int OFF_BAR = OFF_O + 2 * O_TILE;
-constexpr int SMEM_BYTES = OFF_BAR + 256 + 1024;
-constexpr int THREADS = 320;
+constexpr int STAGE = A_TILE + B_TILE;
+constexpr int OFF_BAR = STAGES * STAGE;
+constexpr int SMEM_BYTES = OFF_BAR + 64 + 1024;
+constexpr int THREADS = 256;
 }  // namespace gg
 
 struct GegluParams {
   const __half* bias;   // [2N] or nullptr
+  __half* y;            // [M, N]
   int M, N, K;
-  int m_blocks, n_blocks, k_blocks;
+  int n_blocks, k_blocks;
 };
 
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.f + erff(x * 0.70710678118654752f)); }
 
 __global__ void __launch_bounds__(gg::THREADS, 1)
 ff_geglu_kernel(const __grid_constant__ CUtensorMap tm_a, const __grid_constant__ CUtensorMap tm_b,
-                const __grid_constant__ CUtensorMap tm_y, const __grid_constant__ GegluParams p) {
+                const __grid_constant__ GegluParams p) {
   using namespace gg;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* full = bars;                 // [STAGES] TMA -> MMA
-  uint64_t* empty = bars + STAGES;       // [STAGES] MMA -> TMA
-  uint64_t* acc_full = bars + 2 * STAGES;        // [2] MMA -> epilogue
-  uint64_t* acc_empty = bars + 2 * STAGES + 2;   // [2] epilogue -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + OFF_BAR);   // [STAGES]
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int n_tiles = p.m_blocks * p.n_blocks;
+  const int tid = threadIdx.x, wg = tid >> 7, w = (tid >> 5) & 3, lane = tid & 31;
+  const int m0 = (blockIdx.x / p.n_blocks) * BM, n0 = (blockIdx.x % p.n_blocks) * BN;
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tm_a); tma_prefetch_desc(&tm_b); tma_prefetch_desc(&tm_y);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 256); }
+  auto load = [&](int kb) {   // thread 0
+    const int s = kb % STAGES;
+    uint8_t* st = smem + s * STAGE;
+    mbar_expect_tx(&full[s], STAGE);
+    tma_load_2d(st, &tm_a, &full[s], kb * BK, m0);
+    tma_load_2d(st + A_TILE, &tm_b, &full[s], kb * BK, n0);
+    tma_load_2d(st + A_TILE + B_TILE / 2, &tm_b, &full[s], kb * BK, p.N + n0);
+  };
+  if (tid == 0) {
+    tma_prefetch_desc(&tm_a); tma_prefetch_desc(&tm_b);
+    for (int i = 0; i < STAGES; ++i) mbar_init(&full[i], 1);
     mbar_fence_init();
+    for (int kb = 0; kb < STAGES && kb < p.k_blocks; ++kb) load(kb);
   }
-  if (warp == 1) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t smem_base = smem_u32(smem);
 
-  if (warp == 0) {
-    // ------------------------------------------------------------- TMA producer
-    const uint32_t el = elect_one() ? 1u : 0u;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-      const int m0 = (tile / p.n_blocks) * BM, n0 = (tile % p.n_blocks) * BN;
-      for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
-        const int s = it % STAGES;
-        mbar_wait(&empty[s], ((it / STAGES) & 1) ^ 1);
-        mbar_expect_tx_p(&full[s], A_TILE + B_TILE, el);
-        tma_load_2d_p(smem_base + OFF_A + s * A_TILE, &tm_a, &full[s], kb * BK, m0, el);
-        tma_load_2d_p(smem_base + OFF_B + s * B_TILE, &tm_b, &full[s], kb * BK, n0, el);
-        tma_load_2d_p(smem_base + OFF_B + s * B_TILE + B_TILE / 2, &tm_b, &full[s], kb * BK, p.N + n0, el);
-      }
+  const uint32_t sbase = smem_u32(smem);
+  float v[64], g[64];
+  for (int kb = 0; kb < p.k_blocks; ++kb) {
+    const int s = kb % STAGES;
+    const uint32_t aa = sbase + s * STAGE + wg * 64 * 128;
+    const uint32_t ba = sbase + s * STAGE + A_TILE;
+    mbar_wait(&full[s], (kb / STAGES) & 1);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BK / 16; ++kk) {
+      const uint64_t da = wgmma_desc_sw128(aa + kk * 32, 16, 1024);
+      const uint32_t acc = (kb > 0 || kk > 0) ? 1u : 0u;
+      wgmma_ss<128>(v, da, wgmma_desc_sw128(ba + kk * 32, 16, 1024), acc);
+      wgmma_ss<128>(g, da, wgmma_desc_sw128(ba + B_TILE / 2 + kk * 32, 16, 1024), acc);
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------- MMA issuer
-    const uint32_t el = elect_one() ? 1u : 0u;
-    constexpr uint32_t IDESC = umma_idesc_f16(BM, 2 * BN, 0, 0);
-    const uint64_t da0 = umma_desc_sw128(smem_base + OFF_A, 0, 1024);
-    const uint64_t db0 = umma_desc_sw128(smem_base + OFF_B, 0, 1024);
-    uint32_t it = 0, t = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t) {
-      const uint32_t as = t & 1;
-      mbar_wait(&acc_empty[as], ((t >> 1) & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t acc = tmem + 256u * as;
-      for (int kb = 0; kb < p.k_blocks; ++kb, ++it) {
-        const int s = it % STAGES;
-        mbar_wait(&full[s], (it / STAGES) & 1);
-        tc_fence_after();
-        const uint64_t da = da0 + static_cast<uint64_t>((s * A_TILE) >> 4);
-        const uint64_t db = db0 + static_cast<uint64_t>((s * B_TILE) >> 4);
-#pragma unroll
-        for (int kk = 0; kk < BK / 16; ++kk)
-          mma_f16_ss_p(acc, da + 2 * kk, db + 2 * kk, IDESC, (kb > 0 || kk > 0) ? 1u : 0u, el);
-        tc_commit_p(&empty[s], el);
-      }
-      tc_commit_p(&acc_full[as], el);
-    }
-  } else {
-    // ------------------------------------------------------------- epilogue: thread = output row, 64 columns per warp pair
-    const int ew = warp - 2;
-    const int quad = warp & 3;              // TMEM lane quadrant this warp may access
-    const int half = ew >> 2;               // which 64 output columns
-    const int row = quad * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(quad * 32) << 16;
-    uint8_t* orow = smem + OFF_O + half * O_TILE + row * 128;
-    const int sw = row & 7;
-    const int bar_id = 1 + half;
-    const bool leader = (ew & 3) == 0 && lane == 0;   // one thread per half issues the TMA store
-    uint32_t t = 0;
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++t) {
-      const int m0 = (tile / p.n_blocks) * BM, n0 = (tile % p.n_blocks) * BN;
-      const uint32_t as = t & 1;
-      mbar_wait(&acc_full[as], (t >> 1) & 1);
-      tc_fence_after();
-      const uint32_t acc = tmem + 256u * as + lane_off + 64u * half;
-      if (leader) tma_store_wait_read();                  // the previous tile's store has drained this half's staging tile
-      asm volatile("bar.sync %0, 128;\n" ::"r"(bar_id) : "memory");
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {                       // 32 output columns per pass
-        uint32_t v[32], g[32];
-        tmem_ld32(acc + 32 * c, v);
-        tmem_ld32(acc + 128 + 32 * c, g);
-        tmem_wait_ld_regs32(v);
-        tmem_wait_ld_regs32(g);
-        if (c == 1) {                                     // all TMEM reads of this thread are done: release the accumulator
-          tc_fence_before();
-          mbar_arrive(&acc_empty[as]);
-        }
-        const int col = n0 + 64 * half + 32 * c;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          float bv[8], bg[8];
-          if (p.bias != nullptr) {
-            const uint4 rv = __ldg(reinterpret_cast<const uint4*>(p.bias + col + 8 * q));
-            const uint4 rg = __ldg(reinterpret_cast<const uint4*>(p.bias + p.N + col + 8 * q));
-            const __half2* hv = reinterpret_cast<const __half2*>(&rv);
-            const __half2* hg = reinterpret_cast<const __half2*>(&rg);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 a = __half22float2(hv[i]), b = __half22float2(hg[i]);
-              bv[2 * i] = a.x; bv[2 * i + 1] = a.y; bg[2 * i] = b.x; bg[2 * i + 1] = b.y;
-            }
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) bv[i] = bg[i] = 0.f;
-          }
-          float o[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            o[i] = (__uint_as_float(v[8 * q + i]) + bv[i]) * gelu_erf(__uint_as_float(g[8 * q + i]) + bg[i]);
-          uint4 w;
-          w.x = pack_half2(o[0], o[1]); w.y = pack_half2(o[2], o[3]); w.z = pack_half2(o[4], o[5]); w.w = pack_half2(o[6], o[7]);
-          *reinterpret_cast<uint4*>(orow + (((4 * c + q) ^ sw) << 4)) = w;
-        }
-      }
-      fence_proxy_async_smem();
-      asm volatile("bar.sync %0, 128;\n" ::"r"(bar_id) : "memory");
-      if (leader) {
-        tma_store_2d(&tm_y, smem + OFF_O + half * O_TILE, n0 + 64 * half, m0);
-        tma_store_commit();
-      }
-    }
-    if (leader) tma_store_wait_all();
+    wgmma_commit();
+    wgmma_wait_all<64>(v);
+    pin_regs<64>(g);
+    __syncthreads();   // both warpgroups are done with stage s
+    if (tid == 0 && kb + STAGES < p.k_blocks) load(kb + STAGES);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<512>(tmem);
+
+  // ---- epilogue: bias, erf-GELU, product, fp16, straight from the accumulators
+  const int r0 = m0 + 64 * wg + 16 * w + (lane >> 2), r1 = r0 + 8;
+  const int cq = 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const int col = n0 + 8 * i + cq;
+    float2 bv = make_float2(0.f, 0.f), bg = make_float2(0.f, 0.f);
+    if (p.bias != nullptr) {
+      bv = __half22float2(*reinterpret_cast<const __half2*>(p.bias + col));
+      bg = __half22float2(*reinterpret_cast<const __half2*>(p.bias + p.N + col));
+    }
+    if (r0 < p.M)
+      *reinterpret_cast<__half2*>(p.y + static_cast<size_t>(r0) * p.N + col) =
+          __floats2half2_rn((v[4 * i] + bv.x) * gelu_erf(g[4 * i] + bg.x), (v[4 * i + 1] + bv.y) * gelu_erf(g[4 * i + 1] + bg.y));
+    if (r1 < p.M)
+      *reinterpret_cast<__half2*>(p.y + static_cast<size_t>(r1) * p.N + col) =
+          __floats2half2_rn((v[4 * i + 2] + bv.x) * gelu_erf(g[4 * i + 2] + bg.x), (v[4 * i + 3] + bv.y) * gelu_erf(g[4 * i + 3] + bg.y));
+  }
 }
 
 static int make_2d_map(CUtensorMap* m, const void* ptr, long long rows, long long cols, long long row_stride_elems,
@@ -203,24 +126,17 @@ extern "C" int rtti_ff_geglu_fwd(const void* x, const void* w, const void* bias,
   if (((uintptr_t)x | (uintptr_t)w | (uintptr_t)y | (uintptr_t)bias) & 15) return RTTI_ERR_ALIGN;
   int rc = rtti_arch_ok();
   if (rc != RTTI_OK) return rc;
-  CUtensorMap ta, tb, ty;
+  CUtensorMap ta, tb;
   if ((rc = make_2d_map(&ta, x, m, k, k, gg::BM)) != RTTI_OK) return rc;
   if ((rc = make_2d_map(&tb, w, 2LL * n, k, k, gg::BN)) != RTTI_OK) return rc;
-  if ((rc = make_2d_map(&ty, y, m, n, n, gg::BM)) != RTTI_OK) return rc;
   static const bool configured =
       cudaFuncSetAttribute(ff_geglu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, gg::SMEM_BYTES) == cudaSuccess;
   if (!configured) return RTTI_ERR_CUDA;
-  static const int n_sm = [] {
-    int dev = 0, v = 148;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    return v;
-  }();
   GegluParams p{};
-  p.bias = (const __half*)bias; p.M = (int)m; p.N = n; p.K = k;
-  p.m_blocks = (int)((m + gg::BM - 1) / gg::BM); p.n_blocks = n / gg::BN; p.k_blocks = k / gg::BK;
-  const int tiles = p.m_blocks * p.n_blocks;
-  const int grid = tiles < n_sm ? tiles : n_sm;
-  ff_geglu_kernel<<<grid, gg::THREADS, gg::SMEM_BYTES, (cudaStream_t)stream>>>(ta, tb, ty, p);
+  p.bias = (const __half*)bias; p.y = (__half*)y; p.M = (int)m; p.N = n; p.K = k;
+  p.n_blocks = n / gg::BN; p.k_blocks = k / gg::BK;
+  const long long tiles = ((m + gg::BM - 1) / gg::BM) * p.n_blocks;
+  if (tiles > 0x7fffffffLL) return RTTI_ERR_SHAPE;
+  ff_geglu_kernel<<<(unsigned)tiles, gg::THREADS, gg::SMEM_BYTES, (cudaStream_t)stream>>>(ta, tb, p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

@@ -1,5 +1,5 @@
-// sm_100a PTX wrappers used by the rtti_b200 kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / st / fences) and UMMA descriptor construction.
+// sm_90a PTX wrappers used by the rtti_b200 kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with
+// shared-memory descriptors and register accumulators).
 // Everything here is hand-written inline PTX; no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
@@ -11,16 +11,6 @@ namespace rtti {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}\n"
-      : "=r"(pred));
-  return pred != 0;
 }
 
 // ------------------------------------------------------------------ mbarrier
@@ -79,215 +69,91 @@ __device__ __forceinline__ void tma_store_wait_read() {
 __device__ __forceinline__ void tma_store_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (TMA store / UMMA)
+// generic-proxy smem writes -> visible to the async proxy (TMA store / wgmma)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05 / TMEM
-// A CTA may allocate several times, but not after it has relinquished its allocation permit.
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_keep_permit(uint32_t* smem_result) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {  // whole warp, after the CTA's last allocation
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {  // whole warp; the CTA's only allocation
-  tmem_alloc_keep_permit<kCols>(smem_result);
-  tmem_relinquish();
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory");
-}
-// all previously issued MMAs of this thread arrive (once) on the mbarrier when they complete
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void mma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                           uint32_t accumulate) {
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
-
-// Wait for outstanding tcgen05.ld and tie the destination registers to the wait, so the compiler
-// cannot schedule a consumer of `r` above it.
-__device__ __forceinline__ void tmem_wait_ld_regs32(uint32_t* r) {
-  asm volatile(
-      "tcgen05.wait::ld.sync.aligned;\n"
-      : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-        "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-        "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-        "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-      :
-      : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld_regs16(uint32_t* r) {
-  asm volatile(
-      "tcgen05.wait::ld.sync.aligned;\n"
-      : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-        "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-      :
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
+      " [%0], [%1, {%3, %4}], [%2];\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
 
-// 32 lanes x 32 columns (fp32): thread i of the warp gets lane (base+i), 32 consecutive columns.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-      "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]),
-      "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};\n" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-      : "memory");
-}
-
-// ------------------------------------------------------------------ predicated issue (warp-uniform control warps)
-// A control warp that runs its loop with ALL lanes and predicates only the issuing instructions keeps descriptors and
-// addresses in uniform registers; issuing from inside `if (lane == 0)` makes the compiler wrap every tcgen05 / TMA
-// operand in R2UR + ELECT + BRA.U.ANY sequences (measured: ~1000 SASS instructions per key tile in the 6-member
-// group kernel, which made the single issuing thread the bottleneck). `el` = 1 on the elected lane, 0 elsewhere.
-__device__ __forceinline__ void mbar_expect_tx_p(uint64_t* bar, uint32_t bytes, uint32_t el) {
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t"
-               "@q mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}\n" ::"r"(smem_u32(bar)), "r"(bytes), "r"(el)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_p(uint32_t smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                              int c2, int c3, uint32_t el) {
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %7, 0;\n\t"
-               "@q cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes"
-               " [%0], [%1, {%3, %4, %5, %6}], [%2];\n\t}\n" ::"r"(smem_dst),
-               "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(el)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_p(uint32_t smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
-                                              uint32_t el) {
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-               "@q cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
-               " [%0], [%1, {%3, %4}], [%2];\n\t}\n" ::"r"(smem_dst),
-               "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(el)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tc_commit_p(uint64_t* bar, uint32_t el) {
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %1, 0;\n\t"
-               "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}\n" ::"r"(smem_u32(bar)),
-               "r"(el)
-               : "memory");
-}
-__device__ __forceinline__ void mma_f16_ss_p(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate, uint32_t el) {
-  asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-               "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-               "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(el)
-               : "memory");
-}
-__device__ __forceinline__ void mma_f16_ts_p(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate, uint32_t el) {
-  asm volatile("{\n\t.reg .pred p, q;\n\tsetp.ne.b32 p, %4, 0;\n\tsetp.ne.b32 q, %5, 0;\n\t"
-               "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-               "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(el)
-               : "memory");
-}
-
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor (sm_100 "version 1"), 128-byte swizzle, for tiles whose rows are
-// exactly 128 bytes (64 fp16) and whose 8-row groups are 1024 bytes apart (what TMA SWIZZLE_128B writes).
+// ------------------------------------------------------------------ wgmma (sm_90a warpgroup MMA)
+// Shared-memory matrix descriptor, 128-byte swizzle, for tiles whose rows are exactly 128 bytes (64 fp16) and whose
+// 8-row groups are 1024 bytes apart (what TMA SWIZZLE_128B writes into a 1024-byte aligned tile).
 //   K-major operand  (rows = M or N index, the 64 contiguous elements run along K):
 //       SBO = 1024 B between 8-row groups; LBO unused.     Advance K by 16 elements: +32 B on the start.
 //   MN-major operand (rows = K index, the 64 contiguous elements run along M/N):
 //       SBO = 1024 B between 8-row (K) groups; LBO = byte distance between 64-element MN atoms.
 //       Advance K by 16 rows: +2048 B on the start address.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);          // start address   bits [0,14)
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;     // leading offset  bits [16,30)
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;     // stride offset   bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                             // descriptor version = 1 (Blackwell)
-  d |= static_cast<uint64_t>(2) << 61;                             // layout type: SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                             // layout type: SWIZZLE_128B
   return d;
 }
 
-// Instruction descriptor for kind::f16 with fp16 A/B and fp32 accumulate.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                                   // D format: F32
-         | (0u << 7) | (0u << 10)                    // A, B format: F16
-         | (static_cast<uint32_t>(a_mn_major) << 15) // A major (0 = K)
-         | (static_cast<uint32_t>(b_mn_major) << 16) // B major (0 = K)
-         | (static_cast<uint32_t>(n >> 3) << 17)     // N / 8
-         | (static_cast<uint32_t>(m >> 4) << 24);    // M / 16
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+// Wait for every committed wgmma of this warpgroup, then pin the accumulator registers after the wait so the compiler
+// cannot move a read of them above it.
+template <int N>
+__device__ __forceinline__ void wgmma_wait_all(float* d) {
+  asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory");
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Pin accumulator registers before the first wgmma that reads them (values written by ordinary instructions).
+template <int N>
+__device__ __forceinline__ void pin_regs(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D[64 x N] fp32 (+)= A[64 x 16] * B[16 x N], fp16 operands. `acc` = 0 overwrites D.
+//   wgmma_ss:    A and B from shared memory, both K-major.
+//   wgmma_rs_tb: A from registers (four f16x2 per thread, the m16n8k16 A-fragment layout per warp), B from shared
+//                memory MN-major ("transposed").
+// Accumulator layout per thread (warp w of the warpgroup, lane l): d[4i + {0,1}] = row 16w + l/4, columns
+// 8i + 2(l%4) + {0,1}; d[4i + {2,3}] = row 16w + l/4 + 8, same columns.
+template <int N> __device__ __forceinline__ void wgmma_ss(float* d, uint64_t da, uint64_t db, uint32_t acc);
+template <int N> __device__ __forceinline__ void wgmma_rs_tb(float* d, const uint32_t* a, uint64_t db, uint32_t acc);
+template <> __device__ __forceinline__ void wgmma_ss<64>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc));
+}
+
+template <> __device__ __forceinline__ void wgmma_ss<80>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+      : "l"(da), "l"(db), "r"(acc));
+}
+
+template <> __device__ __forceinline__ void wgmma_ss<128>(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc));
+}
+
+template <> __device__ __forceinline__ void wgmma_rs_tb<64>(float* d, const uint32_t* a, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));
 }
 
 // ------------------------------------------------------------------ misc math
@@ -295,28 +161,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
   return y;
-}
-// two fp16 exponentials per MUFU op (the softmax of head_dim-64 attention is MUFU-bound on B200)
-__device__ __forceinline__ uint32_t ex2_f16x2(uint32_t x) {
-  uint32_t y;
-  asm("ex2.approx.f16x2 %0, %1;\n" : "=r"(y) : "r"(x));
-  return y;
-}
-// packed fp32 pairs (sm_100: FFMA2 / FADD2), one issue slot for two lanes of work
-__device__ __forceinline__ float2 fma_f32x2(float2 a, float2 b, float2 c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;\n"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<const uint64_t*>(&a)), "l"(*reinterpret_cast<const uint64_t*>(&b)),
-        "l"(*reinterpret_cast<const uint64_t*>(&c)));
-  return *reinterpret_cast<float2*>(&d);
-}
-__device__ __forceinline__ float2 add_f32x2(float2 a, float2 b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;\n"
-      : "=l"(d)
-      : "l"(*reinterpret_cast<const uint64_t*>(&a)), "l"(*reinterpret_cast<const uint64_t*>(&b)));
-  return *reinterpret_cast<float2*>(&d);
 }
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);

@@ -17,17 +17,6 @@ int encode_tiled_f16(CUtensorMap* map, const void* base, int rank, const cuuint6
 int make_head_map(CUtensorMap* m, const void* ptr, int head_dim, int heads, int rows, int batch, long long bs,
                   long long rs, int box_rows);
 
-// attn_self.cu: self-attention for head_dim <= 64 (Q/O maps with 128-row boxes, K/V maps with 64-row boxes). Batch entries
-// with the same qk_src share one softmax (groups of up to `max_group` <= 6 members per CTA).
-int launch_attn_self(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& to,
-                     int batch, int heads, int head_dim, int n_q, int n_k, float scale_log2, const int8_t* qk_src,
-                     float* lse, int max_group, cudaStream_t stream);
-
-// attn_cross.cu: 77-key cross-attention for head_dim <= 64 without capture (Q/O maps: 128-row boxes, K/V maps: 80-row boxes)
-int launch_attn_cross(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& to,
-                      int batch, int heads, int head_dim, int n_q, int n_k, float scale_log2, unsigned long long fs_mask,
-                      const int* word_pos, const float* font_size, int n_fs, cudaStream_t stream);
-
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
 }  // namespace rtti

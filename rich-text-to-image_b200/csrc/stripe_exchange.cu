@@ -92,7 +92,7 @@ extern "C" int rtti_halo_exchange(float* pad_local, float* pad_up, float* pad_do
   if (((uintptr_t)pad_local | (uintptr_t)pad_up | (uintptr_t)pad_down) & 15) return RTTI_ERR_ALIGN;
   const long long row_vec = row_elems / 4;
   long long blocks = (row_vec + 255) / 256;
-  if (blocks > 148) blocks = 148;
+  if (blocks > 132) blocks = 132;
   halo_exchange_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(pad_local, pad_up, pad_down, rows, row_vec,
                                                                       (unsigned int*)flags_local, (unsigned int*)flags_up,
                                                                       (unsigned int*)flags_down, seq);

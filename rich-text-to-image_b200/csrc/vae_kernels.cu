@@ -19,7 +19,7 @@ static GN32Plan gn32_plan(int batch, int hw, int c) {
   p.nvec = c / 4;
   p.rowlanes = p.nvec >= 256 ? 1 : (256 / p.nvec);
   p.threads = p.nvec * p.rowlanes;
-  int want = (148 * 8 + batch - 1) / batch;
+  int want = (132 * 8 + batch - 1) / batch;
   int maxc = (hw + p.rowlanes * 8 - 1) / (p.rowlanes * 8);  // at least 8 rows per thread
   if (maxc < 1) maxc = 1;
   p.chunks = want < maxc ? want : maxc;
@@ -427,7 +427,7 @@ extern "C" int rtti_add_bias_f32(const float* a, const float* b, const float* bi
   if (((uintptr_t)a | (uintptr_t)b | (uintptr_t)out | (uintptr_t)bias) & 15) return RTTI_ERR_ALIGN;
   const long long nvec = rows * (c / 4);
   long long blocks = (nvec + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   add_bias_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(a, b, bias, out, nvec, c / 4);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

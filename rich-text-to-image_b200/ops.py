@@ -14,7 +14,7 @@ _F16 = torch.float16
 
 # number of kernels of librtti_b200.so launched since import (bench.py reports the count of a timed region)
 LAUNCHES = 0
-# feed-forward input projection: True = rtti_ff_geglu_fwd (hand-written tcgen05 GEMM with the gate in its epilogue),
+# feed-forward input projection: True = rtti_ff_geglu_fwd (hand-written wgmma GEMM with the gate in its epilogue),
 # False = cuBLAS GEMM + rtti_geglu_fwd (kept for A/B measurements, profiles/)
 FUSED_FF_GEGLU = True
 # when a list: attention() appends (start_event, end_event, kind, flops, algorithmic_bytes) per launch
@@ -190,7 +190,7 @@ def add_bias_layernorm(a, resid, bias, gamma, beta, eps, h_out=None, y=None):
 
 
 def ff_geglu(x, weight, bias=None, out=None):
-    """(x W_v^T + b_v) * gelu(x W_g^T + b_g) with weight [2n, k] = [W_v; W_g] (rtti_ff_geglu_fwd: tcgen05 GEMM with the
+    """(x W_v^T + b_v) * gelu(x W_g^T + b_g) with weight [2n, k] = [W_v; W_g] (rtti_ff_geglu_fwd: wgmma GEMM with the
     gate in the epilogue). x [..., k] fp16 contiguous -> [..., n]."""
     lib = _lib.load()
     _req(x, _F16, "x"); _req(weight, _F16, "weight")

@@ -1,4 +1,4 @@
-"""RegionDiffusion (SD1.5) — B200-native drop-in for models/region_diffusion.py of the reference.
+"""RegionDiffusion (SD1.5) — H100 drop-in for models/region_diffusion.py of the reference.
 
 Public surface kept: `RegionDiffusion(device)`, `produce_attn_maps`, `produce_latents`, `prompt_to_img`,
 `predict_x0`, `register_tokenmap_hooks / remove_tokenmap_hooks`, attributes `.unet .vae .tokenizer

@@ -1,4 +1,4 @@
-"""RegionDiffusionXL — B200-native drop-in for models/region_diffusion_sdxl.py of the reference.
+"""RegionDiffusionXL — H100 drop-in for models/region_diffusion_sdxl.py of the reference.
 
 Same public surface (`sample(...)`, `register_tokenmap_hooks / remove_tokenmap_hooks`, `.masks`,
 `.selfattn_maps / .crossattn_maps / .n_maps`, `.unet .vae .scheduler .tokenizer`) and the same per-step

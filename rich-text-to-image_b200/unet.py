@@ -1,4 +1,4 @@
-"""B200-native UNet2DConditionModel for the region-diffusion sampler.
+"""UNet2DConditionModel on the H100 kernels for the region-diffusion sampler.
 
 Mirrors the interface and parameter names of the reference's patched UNet (models/unet_2d_condition.py:703-983,
 unet_2d_blocks.py, transformer_2d.py:270-310, attention.py:131-206, resnet.py:591-645) so diffusers-format
@@ -6,7 +6,7 @@ checkpoints load unchanged, but is organised for the hardware instead of for hoo
 
   * activations are channels-last fp16 `[B, H*W, C]` end to end (no NCHW<->NHWC permute copies around the
     transformers, cuDNN NHWC tensor-core convolutions);
-  * every normalisation / gating op and both attentions run in the hand-written sm_100a kernels of
+  * every normalisation / gating op and both attentions run in the hand-written sm_90a kernels of
     librtti_b200.so (ops.py); GEMMs and 3x3 convolutions are plain library calls (cuBLASLt / cuDNN);
   * the reference's per-pass PyTorch hooks (token-map capture, self-attention / feature injection,
     font-size re-weighting; models/region_diffusion_sdxl.py:959-1140) are a `RegionControl` argument:

@@ -6,12 +6,12 @@ weight gradients it never uses. Here the decoder (vae.py, diffusers parameter na
 static sequence — no autograd graph, no autograd thread, CUDA-graph capturable:
 
   * channels-last fp32 activations [B, H*W, C] end to end;
-  * GroupNorm(+SiLU) forward and backward in the sm_100a kernels of csrc/vae_kernels.cu
+  * GroupNorm(+SiLU) forward and backward in the sm_90a kernels of csrc/vae_kernels.cu
     (PyTorch's native GroupNorm round-trips channels-last tensors through NCHW copies);
   * 3x3 / 1x1 convolutions: cuDNN forward and `convolution_backward` with output_mask=(True, False, False)
     (data gradient only, TF32 tensor cores as in the reference's default PyTorch settings);
   * the single-head 16384-token mid-block attention materialises its 1 GB probability matrix once
-    (B200: 180 GB) and reuses it for the five backward GEMMs instead of recomputing it.
+    and reuses it for the five backward GEMMs instead of recomputing it.
 """
 import math
 

@@ -1,5 +1,5 @@
 """sample.py — command-line entry with the reference's flags (sample.py:117-134 of the reference), driving
-the B200-native samplers. Flow = reference sample.py:17-114: parse the rich-text JSON, plain pass with token-map
+the H100 samplers. Flow = reference sample.py:17-114: parse the rich-text JSON, plain pass with token-map
 capture, get_token_maps (twice: colour masks, region masks), rich-text pass.
 
 Extra flags: --load_path (LOCAL diffusers-format directory; there is no hub access in this environment) and

@@ -1,4 +1,4 @@
-"""Honest GPU baseline (SURVEY §8d): the reference's algorithm as plain PyTorch-eager on the SAME B200 —
+"""Honest GPU baseline (SURVEY §8d): the reference's algorithm as plain PyTorch-eager on the SAME GPU —
 the oracle restatement (oracle/unet_oracle.py: baddbmm -> softmax -> bmm with the probability tensor
 materialised, head mean on every call, batch-1 passes run one after another as models/region_diffusion_sdxl.py:787-821
 does), fp16 weights. Times UNet passes only (8 per step for the 5-region injected workload); prints one JSON line.

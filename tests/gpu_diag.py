@@ -181,7 +181,7 @@ def case_elementwise():
 
 
 def case_ff_geglu():
-    """tcgen05 GEMM with the GEGLU gate in the epilogue against torch (fp32 matmul of the fp16 operands)."""
+    """wgmma GEMM with the GEGLU gate in the epilogue against torch (fp32 matmul of the fp16 operands)."""
     import torch
     from rtti_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(2)

@@ -97,7 +97,7 @@ def main():
             yo = torch.empty(rows, 4 * C, device="cuda", dtype=torch.float16)
             fl = 2.0 * rows * C * 8 * C
             sec = timeit(lambda: ops.ff_geglu(x, w, bb, out=yo))
-            report(f"ff_geglu (tcgen05 GEMM + gate epilogue) rows{rows} C{C}", sec, flops=fl, bound="tensor")
+            report(f"ff_geglu (wgmma GEMM + gate epilogue) rows{rows} C{C}", sec, flops=fl, bound="tensor")
             sec = timeit(lambda: ops.geglu(torch.nn.functional.linear(x, w, bb), out=yo))
             report(f"cuBLAS linear + geglu kernel rows{rows} C{C}", sec, flops=fl, bound="tensor")
             sec = timeit(lambda: torch.nn.functional.linear(x, w, bb))
@@ -119,7 +119,7 @@ def main():
         yo = torch.empty(rows, 4 * C, device="cuda", dtype=torch.float16)
         fl = 2.0 * rows * C * 8 * C
         sec = timeit(lambda: ops.ff_geglu(x, w, bb, out=yo))
-        report(f"ff_geglu (tcgen05 GEMM + gate epilogue) rows{rows} C{C}", sec, flops=fl, bound="tensor")
+        report(f"ff_geglu (wgmma GEMM + gate epilogue) rows{rows} C{C}", sec, flops=fl, bound="tensor")
         sec = timeit(lambda: ops.geglu(torch.nn.functional.linear(x, w, bb), out=yo))
         report(f"cuBLAS linear + geglu kernel rows{rows} C{C}", sec, flops=fl, bound="tensor")
         sec = timeit(lambda: torch.nn.functional.linear(x, w, bb))

@@ -1,4 +1,4 @@
-"""CPU: checkpoints in the diffusers on-disk layout load into the B200 modules (rtti_b200/loading.py) — the drop-in claim
+"""CPU: checkpoints in the diffusers on-disk layout load into the rtti_b200 modules (rtti_b200/loading.py) — the drop-in claim
 for real weights (the reference downloads them from the hub: models/region_diffusion.py:24-33, region_diffusion_sdxl.py:105-120)."""
 import json
 import os
