@@ -151,14 +151,27 @@ int rtti_predict_x0(const void* x_t, const void* eps, float alpha, void* x0, lon
  * mean_rstd [batch, groups, 2] fp32 (written by fwd, read by bwd); workspace fp32
  * [rtti_gn32_workspace_elems(...)]. dx = d loss / d x given dz = d loss / d (silu?(GN(x))).
  * chan_bias: optional fp32 [c] added to x first (the bias of the convolution that produced x, folded in); NULL to skip.
+ * addend (bwd): optional fp32 [batch, hw, c] added to dx (the gradient reaching a resnet block's shortcut path); NULL
+ * to skip.
  */
 long long rtti_gn32_workspace_elems(int batch, int hw, int c, int groups);
 int rtti_gn32_silu_fwd(const float* x, const float* chan_bias, const float* gamma, const float* beta, float* y,
                        float* mean_rstd, float* workspace, int batch, int hw, int c, int groups, float eps,
                        int apply_silu, void* stream);
 int rtti_gn32_silu_bwd(const float* x, const float* chan_bias, const float* dz, const float* gamma, const float* beta,
-                       const float* mean_rstd, float* dx, float* workspace, int batch, int hw, int c, int groups,
-                       int apply_silu, void* stream);
+                       const float* mean_rstd, const float* addend, float* dx, float* workspace, int batch, int hw,
+                       int c, int groups, int apply_silu, void* stream);
+/* Nearest x2 upsample + 3x3 convolution of the VAE decoder (diffusers Upsample2D) evaluated at low resolution:
+ * output pixel (2i+a, 2j+b) only sees low-res rows {i-1, i} (a = 0) or {i, i+1} (a = 1), likewise for columns, so
+ * the layer is one 2x2, pad-1 convolution of the low-res input x [batch, h, w, c] with the four phase-folded filters
+ * stacked along the output channels, y4 [batch, h+1, w+1, 4c] (phase k = 2a+b of pixel (i, j) at (i+a, j+b),
+ * channels k*c..k*c+c-1): 16 instead of 36 multiply-adds per (output pixel, cin, cout).
+ * rtti_upsample_phase_interleave: out [batch, 2h, 2w, c] = y4 re-ordered to pixels + bias[c] (bias may be NULL).
+ * rtti_upsample_phase_scatter: its adjoint, g [batch, 2h, 2w, c] -> dy4 [batch, h+1, w+1, 4c] (zero where the
+ * interleave reads nothing). fp32, c a multiple of 4, 16-byte aligned. */
+int rtti_upsample_phase_interleave(const float* y4, const float* bias, float* out, int batch, int h, int w, int c,
+                                   void* stream);
+int rtti_upsample_phase_scatter(const float* g, float* dy4, int batch, int h, int w, int c, void* stream);
 /* out[rows, c] = a + b + bias[c] (fp32): the residual add of a VAE resnet block fused with the bias of the
  * convolution that produced b; bias may be NULL. */
 int rtti_add_bias_f32(const float* a, const float* b, const float* bias, float* out, long long rows, int c,

@@ -44,8 +44,10 @@ SIGNATURES = {
     "rtti_predict_x0": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_ll, c_void_p]),
     "rtti_gn32_workspace_elems": (c_ll, [c_int] * 4),
     "rtti_gn32_silu_fwd": (c_int, [c_void_p] * 7 + [c_int] * 4 + [c_float, c_int, c_void_p]),
-    "rtti_gn32_silu_bwd": (c_int, [c_void_p] * 8 + [c_int] * 4 + [c_int, c_void_p]),
+    "rtti_gn32_silu_bwd": (c_int, [c_void_p] * 9 + [c_int] * 4 + [c_int, c_void_p]),
     "rtti_add_bias_f32": (c_int, [c_void_p] * 4 + [c_ll, c_int, c_void_p]),
+    "rtti_upsample_phase_interleave": (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_void_p]),
+    "rtti_upsample_phase_scatter": (c_int, [c_void_p] * 2 + [c_int] * 4 + [c_void_p]),
     "rtti_gather_blend_step": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int, c_int, c_int,
                                        c_void_p, c_ll, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float,
                                        ctypes.c_uint, c_void_p]),

@@ -148,12 +148,14 @@ __global__ void gn32_finalize_kernel(const float* __restrict__ ws, float* __rest
   }
 }
 
-// MODE 0: y = silu?(xhat*gamma+beta).  MODE 1: dx = rstd*(dy*gamma - c1 - xhat*c2)
+// MODE 0: y = silu?(xhat*gamma+beta).  MODE 1: dx = rstd*(dy*gamma - c1 - xhat*c2) (+ addend, e.g. the gradient
+// reaching a resnet's identity / shortcut path, so the block's input gradient needs no separate add pass)
 template <int MODE>
 __global__ void gn32_apply_kernel(const float* __restrict__ x, const float* __restrict__ cbias,
                                   const float* __restrict__ dz,
                                   const float* __restrict__ gamma, const float* __restrict__ beta,
                                   const float* __restrict__ mean_rstd, const float* __restrict__ c12,
+                                  const float* __restrict__ addend,
                                   float* __restrict__ out, int hw, int c, int groups, int nvec, int rowlanes,
                                   int rows_per_chunk, int silu) {
   const int b = blockIdx.y, chunk = blockIdx.x;
@@ -200,6 +202,14 @@ __global__ void gn32_apply_kernel(const float* __restrict__ x, const float* __re
     }
     return make_float4(o[0], o[1], o[2], o[3]);
   };
+  auto store = [&](int row, float4 v) {
+    const size_t off = base + (size_t)row * c;
+    if (MODE == 1 && addend) {
+      const float4 a = *reinterpret_cast<const float4*>(addend + off);
+      v.x += a.x; v.y += a.y; v.z += a.z; v.w += a.w;
+    }
+    *reinterpret_cast<float4*>(out + off) = v;
+  };
   int r = r0 + rl;
   for (; r + 3 * rowlanes < r1; r += 4 * rowlanes) {
     float4 xv[4], dv[4];
@@ -209,14 +219,13 @@ __global__ void gn32_apply_kernel(const float* __restrict__ x, const float* __re
       if (MODE == 1) dv[u] = *reinterpret_cast<const float4*>(dz + base + (size_t)(r + u * rowlanes) * c);
     }
 #pragma unroll
-    for (int u = 0; u < 4; ++u)
-      *reinterpret_cast<float4*>(out + base + (size_t)(r + u * rowlanes) * c) = apply(xv[u], dv[u]);
+    for (int u = 0; u < 4; ++u) store(r + u * rowlanes, apply(xv[u], dv[u]));
   }
   for (; r < r1; r += rowlanes) {
     const float4 xv = *reinterpret_cast<const float4*>(x + base + (size_t)r * c);
     float4 dv = xv;
     if (MODE == 1) dv = *reinterpret_cast<const float4*>(dz + base + (size_t)r * c);
-    *reinterpret_cast<float4*>(out + base + (size_t)r * c) = apply(xv, dv);
+    store(r, apply(xv, dv));
   }
 }
 
@@ -329,17 +338,18 @@ extern "C" int rtti_gn32_silu_fwd(const float* x, const float* chan_bias, const 
                                                         p.nvec, p.rowlanes, p.rows_per_chunk, p.chunks, 0);
   gn32_finalize_kernel<0><<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, mean_rstd, groups, p.chunks,
                                                                          (float)hw * (float)(c / groups), eps);
-  gn32_apply_kernel<0><<<grid, p.threads, 0, st>>>(x, chan_bias, nullptr, gamma, beta, mean_rstd, nullptr, y, hw, c, groups,
-                                                   p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
+  gn32_apply_kernel<0><<<grid, p.threads, 0, st>>>(x, chan_bias, nullptr, gamma, beta, mean_rstd, nullptr, nullptr, y, hw, c,
+                                                   groups, p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }
 
 extern "C" int rtti_gn32_silu_bwd(const float* x, const float* chan_bias, const float* dz, const float* gamma, const float* beta,
-                                  const float* mean_rstd, float* dx, float* workspace, int batch, int hw, int c,
-                                  int groups, int apply_silu, void* stream) {
+                                  const float* mean_rstd, const float* addend, float* dx, float* workspace, int batch,
+                                  int hw, int c, int groups, int apply_silu, void* stream) {
   int rc = gn32_check(x, gamma, beta, dx, batch, hw, c, groups);
   if (rc != RTTI_OK) return rc;
   if (!dz || !mean_rstd || !workspace || ((uintptr_t)dz & 15)) return RTTI_ERR_ARG;
+  if ((uintptr_t)addend & 15) return RTTI_ERR_ALIGN;
   const GN32Plan p = gn32_plan(batch, hw, c);
   const size_t smem = (size_t)p.rowlanes * c * 2 * sizeof(float);
   if (smem > 48 * 1024) return RTTI_ERR_SHAPE;
@@ -350,8 +360,8 @@ extern "C" int rtti_gn32_silu_bwd(const float* x, const float* chan_bias, const 
                                                         p.rowlanes, p.rows_per_chunk, p.chunks, apply_silu);
   gn32_finalize_kernel<1><<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, c12, groups, p.chunks,
                                                                          (float)hw * (float)(c / groups), 0.f);
-  gn32_apply_kernel<1><<<grid, p.threads, 0, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, c12, dx, hw, c, groups, p.nvec,
-                                                   p.rowlanes, p.rows_per_chunk, apply_silu);
+  gn32_apply_kernel<1><<<grid, p.threads, 0, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, c12, addend, dx, hw, c, groups,
+                                                   p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }
 
@@ -376,8 +386,8 @@ extern "C" int rtti_gn32_silu_fwd_striped(const float* x, const float* chan_bias
                                                         groups, p.nvec, p.rowlanes, p.rows_per_chunk, p.chunks, 0);
   gn32_finalize_peer_kernel<0><<<1, 32 * groups, 0, st>>>(workspace, mean_rstd, pp, groups, p.chunks,
                                                           (float)hw_total * (float)(c / groups), eps);
-  gn32_apply_kernel<0><<<grid, p.threads, 0, st>>>(x, chan_bias, nullptr, gamma, beta, mean_rstd, nullptr, y, hw_local, c,
-                                                   groups, p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
+  gn32_apply_kernel<0><<<grid, p.threads, 0, st>>>(x, chan_bias, nullptr, gamma, beta, mean_rstd, nullptr, nullptr, y, hw_local,
+                                                   c, groups, p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }
 
@@ -403,8 +413,8 @@ extern "C" int rtti_gn32_silu_bwd_striped(const float* x, const float* chan_bias
                                                         groups, p.nvec, p.rowlanes, p.rows_per_chunk, p.chunks, apply_silu);
   gn32_finalize_peer_kernel<1><<<1, 32 * groups, 0, st>>>(workspace, c12, pp, groups, p.chunks,
                                                           (float)hw_total * (float)(c / groups), 0.f);
-  gn32_apply_kernel<1><<<grid, p.threads, 0, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, c12, dx, hw_local, c, groups,
-                                                   p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
+  gn32_apply_kernel<1><<<grid, p.threads, 0, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, c12, nullptr, dx, hw_local, c,
+                                                   groups, p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }
 
@@ -429,5 +439,81 @@ extern "C" int rtti_add_bias_f32(const float* a, const float* b, const float* bi
   long long blocks = (nvec + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;
   add_bias_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(a, b, bias, out, nvec, c / 4);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+// ---- nearest x2 upsample + 3x3 convolution, evaluated at low resolution --------------------------------------------
+// High-res output pixel (2i+a, 2j+b) of conv3x3(upsample2x(x)) is a 2x2 convolution of the low-res x with a folded
+// filter per phase (a, b). One 2x2, pad-1 convolution with the four folded filters stacked along Cout yields
+// y4 [B, h+1, w+1, 4c], where phase k = 2a+b of pixel (i, j) sits at low-res position (i+a, j+b), channels k*c.
+// These two kernels move between that layout and the high-res tensor [B, 2h, 2w, c].
+
+// out[b, 2i+a, 2j+bb, ch] = y4[b, i+a, j+bb, (2a+bb)*c + ch] + bias[ch]
+__global__ void upsample_phase_interleave_kernel(const float* __restrict__ y4, const float* __restrict__ bias,
+                                                 float* __restrict__ out, long long nvec, int h, int w, int cvec) {
+  const int H = 2 * h, W = 2 * w;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % cvec);
+    long long pix = i / cvec;
+    const int x = (int)(pix % W); pix /= W;
+    const int y = (int)(pix % H);
+    const long long b = pix / H;
+    const int a = y & 1, bb = x & 1;
+    const long long src = ((b * (h + 1) + (y >> 1) + a) * (w + 1) + (x >> 1) + bb) * (4LL * cvec) + (2 * a + bb) * cvec + cv;
+    float4 v = reinterpret_cast<const float4*>(y4)[src];
+    if (bias) {
+      const float4 z = reinterpret_cast<const float4*>(bias)[cv];
+      v.x += z.x; v.y += z.y; v.z += z.z; v.w += z.w;
+    }
+    reinterpret_cast<float4*>(out)[i] = v;
+  }
+}
+
+// adjoint of the interleave: dy4[b, p, q, (2a+bb)*c + ch] = g[b, 2(p-a)+a, 2(q-bb)+bb, ch], 0 where (p-a, q-bb) falls
+// outside the low-res image (those positions of y4 are never read by the interleave)
+__global__ void upsample_phase_scatter_kernel(const float* __restrict__ g, float* __restrict__ dy4, long long nvec, int h,
+                                              int w, int cvec) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (long long)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % (4 * cvec));
+    long long pix = i / (4 * cvec);
+    const int q = (int)(pix % (w + 1)); pix /= (w + 1);
+    const int p = (int)(pix % (h + 1));
+    const long long b = pix / (h + 1);
+    const int k = cv / cvec, a = k >> 1, bb = k & 1;
+    const int li = p - a, lj = q - bb;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (li >= 0 && li < h && lj >= 0 && lj < w)
+      v = reinterpret_cast<const float4*>(g)[((b * 2 * h + 2 * li + a) * (2LL * w) + 2 * lj + bb) * cvec + cv % cvec];
+    reinterpret_cast<float4*>(dy4)[i] = v;
+  }
+}
+
+static int upsample_phase_check(const void* a, const void* b, int batch, int h, int w, int c) {
+  if (!a || !b || batch < 1 || h < 1 || w < 1 || c < 4) return RTTI_ERR_ARG;
+  if (c % 4 != 0) return RTTI_ERR_SHAPE;
+  if (((uintptr_t)a | (uintptr_t)b) & 15) return RTTI_ERR_ALIGN;
+  return RTTI_OK;
+}
+
+static int elementwise_blocks(long long nvec) {
+  const long long blocks = (nvec + 255) / 256;
+  return (int)(blocks < 132 * 16 ? blocks : 132 * 16);
+}
+
+extern "C" int rtti_upsample_phase_interleave(const float* y4, const float* bias, float* out, int batch, int h, int w, int c,
+                                              void* stream) {
+  int rc = upsample_phase_check(y4, out, batch, h, w, c);
+  if (rc != RTTI_OK) return rc;
+  if ((uintptr_t)bias & 15) return RTTI_ERR_ALIGN;
+  const long long nvec = (long long)batch * 4 * h * w * (c / 4);
+  upsample_phase_interleave_kernel<<<elementwise_blocks(nvec), 256, 0, (cudaStream_t)stream>>>(y4, bias, out, nvec, h, w, c / 4);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+extern "C" int rtti_upsample_phase_scatter(const float* g, float* dy4, int batch, int h, int w, int c, void* stream) {
+  int rc = upsample_phase_check(g, dy4, batch, h, w, c);
+  if (rc != RTTI_OK) return rc;
+  const long long nvec = (long long)batch * (h + 1) * (w + 1) * c;
+  upsample_phase_scatter_kernel<<<elementwise_blocks(nvec), 256, 0, (cudaStream_t)stream>>>(g, dy4, nvec, h, w, c / 4);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

@@ -358,15 +358,18 @@ def gn32_silu_fwd(x, gamma, beta, groups, eps, silu, chan_bias=None):
     return y, stats
 
 
-def gn32_silu_bwd(x, dz, gamma, beta, stats, groups, silu, chan_bias=None):
-    """Input gradient of gn32_silu_fwd (rtti_gn32_silu_bwd)."""
+def gn32_silu_bwd(x, dz, gamma, beta, stats, groups, silu, chan_bias=None, addend=None):
+    """Input gradient of gn32_silu_fwd (rtti_gn32_silu_bwd); `addend` (same shape as x) is added to it."""
     lib = _lib.load()
     _req(x, torch.float32, "x"); _req(dz, torch.float32, "dz")
     assert x.is_contiguous() and dz.is_contiguous() and dz.shape == x.shape
+    if addend is not None:
+        _req(addend, torch.float32, "addend")
+        assert addend.is_contiguous() and addend.shape == x.shape
     B, HW, C = x.shape
     dx = torch.empty_like(x)
-    rc = lib.rtti_gn32_silu_bwd(_ptr(x), _ptr(chan_bias), _ptr(dz), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(dx),
-                                _ptr(_gn32_workspace(x, groups)), B, HW, C, groups, 1 if silu else 0, _stream())
+    rc = lib.rtti_gn32_silu_bwd(_ptr(x), _ptr(chan_bias), _ptr(dz), _ptr(gamma), _ptr(beta), _ptr(stats), _ptr(addend),
+                                _ptr(dx), _ptr(_gn32_workspace(x, groups)), B, HW, C, groups, 1 if silu else 0, _stream())
     _lib.check(rc, "rtti_gn32_silu_bwd")
     _count(3)
     return dx
@@ -462,6 +465,35 @@ def add_bias_f32(a, b, bias=None, out=None):
     _lib.check(lib.rtti_add_bias_f32(_ptr(a), _ptr(b), _ptr(bias), _ptr(out), a.numel() // C, C, _stream()), "rtti_add_bias_f32")
     _count(1)
     return out
+
+
+def upsample_phase_interleave(y4, bias, h, w):
+    """y4 [B, (h+1)*(w+1), 4C] (2x2 pad-1 convolution with the phase-folded filters of an upsampler, vae_guidance)
+    -> [B, 4*h*w, C] high-res output + bias[C] (rtti_upsample_phase_interleave)."""
+    lib = _lib.load()
+    _req(y4, torch.float32, "y4")
+    B, n, C4 = y4.shape
+    assert y4.is_contiguous() and n == (h + 1) * (w + 1) and C4 % 4 == 0
+    C = C4 // 4
+    if bias is not None:
+        _req(bias, torch.float32, "bias"); assert bias.is_contiguous() and bias.numel() == C
+    out = torch.empty(B, 4 * h * w, C, dtype=torch.float32, device=y4.device)
+    _lib.check(lib.rtti_upsample_phase_interleave(_ptr(y4), _ptr(bias), _ptr(out), B, h, w, C, _stream()),
+               "rtti_upsample_phase_interleave")
+    _count(1)
+    return out
+
+
+def upsample_phase_scatter(g, h, w):
+    """Adjoint of upsample_phase_interleave: g [B, 4*h*w, C] -> [B, (h+1)*(w+1), 4C] (rtti_upsample_phase_scatter)."""
+    lib = _lib.load()
+    _req(g, torch.float32, "g")
+    B, n, C = g.shape
+    assert g.is_contiguous() and n == 4 * h * w
+    dy4 = torch.empty(B, (h + 1) * (w + 1), 4 * C, dtype=torch.float32, device=g.device)
+    _lib.check(lib.rtti_upsample_phase_scatter(_ptr(g), _ptr(dy4), B, h, w, C, _stream()), "rtti_upsample_phase_scatter")
+    _count(1)
+    return dy4
 
 
 def add_bias_f16(a, b, bias=None, out=None):

@@ -10,6 +10,10 @@ static sequence — no autograd graph, no autograd thread, CUDA-graph capturable
     (PyTorch's native GroupNorm round-trips channels-last tensors through NCHW copies);
   * 3x3 / 1x1 convolutions: cuDNN forward and `convolution_backward` with output_mask=(True, False, False)
     (data gradient only, TF32 tensor cores as in the reference's default PyTorch settings);
+  * nearest x2 upsample + 3x3 convolution evaluated at low resolution: each output phase is a 2x2 convolution with a
+    folded filter, so the layer is one 2x2 convolution of the low-res input with the four folded filters stacked
+    (16 instead of 36 multiply-adds per output element, no 4x upsampled copy); its output is interleaved into the
+    high-res tensor (and the gradient scattered back) by csrc/vae_kernels.cu;
   * the single-head 16384-token mid-block attention materialises its 1 GB probability matrix once
     and reuses it for the five backward GEMMs instead of recomputing it.
 """
@@ -21,6 +25,11 @@ import torch.nn.functional as F
 from . import ops
 
 _conv_bwd = torch.ops.aten.convolution_backward
+
+# _PHASE_TAPS[a][t][k]: weight of 3x3 kernel row k in tap t of output phase a (rows 2i+a of the x2 nearest upsample
+# read low-res rows i-1, i, i (a = 0) or i, i, i+1 (a = 1)); tap t of the 2x2, pad-1 phase convolution at low-res
+# output position p reads row p-1+t, and phase a of row i sits at p = i+a. Columns likewise.
+_PHASE_TAPS = (((1., 0., 0.), (0., 1., 1.)), ((1., 1., 0.), (0., 0., 1.)))
 
 
 class _Tape(list):
@@ -55,6 +64,7 @@ class DecoderFwdBwd:
         self.vae = vae
         self.groups = vae.config.norm_num_groups
         self._dummies = {}
+        self._wphase = {}
 
     # ------------------------------------------------------------------ pieces
     def _gn_f(self, norm, x, silu, tape, chan_bias=None):
@@ -62,9 +72,10 @@ class DecoderFwdBwd:
         tape.append(("gn", norm, x, stats, silu, chan_bias))
         return y
 
-    def _gn_b(self, rec, g):
+    def _gn_b(self, rec, g, addend=None):
         _, norm, x, stats, silu, chan_bias = rec
-        return ops.gn32_silu_bwd(x, g.contiguous(), norm.weight, norm.bias, stats, self.groups, silu, chan_bias=chan_bias)
+        return ops.gn32_silu_bwd(x, g.contiguous(), norm.weight, norm.bias, stats, self.groups, silu, chan_bias=chan_bias,
+                                 addend=addend)
 
     def _dummy(self, shape, dev):
         k = (tuple(shape), str(dev))
@@ -76,6 +87,31 @@ class DecoderFwdBwd:
         g4 = _nchw(g, H, W)
         gi, _, _ = _conv_bwd(g4, self._dummy((g.shape[0], cin, H, W), g.device), conv.weight, None, list(conv.stride),
                              list(conv.padding), [1, 1], False, [0, 0], 1, [True, False, False])
+        return _cl(gi)[0]
+
+    def _phase_filter(self, conv):
+        """[4*Cout, Cin, 2, 2] channels-last: the 3x3 filter of an upsampler folded into its four output phases,
+        phase 2a+b in output channels (2a+b)*Cout.. (computed once per VAE in fp64: the weights are frozen).
+        The fold is cached per module and never refreshed: changing conv.weight in place after the first call (e.g.
+        load_state_dict) is not seen; build a new engine (vae._fwd_bwd = None) after loading other weights."""
+        hit = self._wphase.get(id(conv))
+        if hit is None or hit[0] is not conv:   # the module is kept with its filter: an id can be reused
+            w = conv.weight.double()
+            taps = torch.tensor(_PHASE_TAPS, dtype=w.dtype, device=w.device)
+            wf = torch.einsum("atk,bul,oikl->aboitu", taps, taps, w).reshape(4 * w.shape[0], w.shape[1], 2, 2)
+            hit = self._wphase[id(conv)] = (conv, wf.float().contiguous(memory_format=torch.channels_last))
+        return hit[1]
+
+    def _upsample_f(self, conv, x, H, W):
+        """conv3x3(nearest_x2(x)) for x [B, H*W, C] -> [B, 4*H*W, Cout]."""
+        y4 = F.conv2d(_nchw(x, H, W), self._phase_filter(conv), None, 1, 1)
+        return ops.upsample_phase_interleave(_cl(y4)[0], conv.bias, H, W)
+
+    def _upsample_b(self, conv, g, H, W, C):
+        """Input gradient of _upsample_f: g [B, 4*H*W, Cout] -> [B, H*W, C]."""
+        dy4 = ops.upsample_phase_scatter(g.contiguous(), H, W)
+        gi, _, _ = _conv_bwd(_nchw(dy4, H + 1, W + 1), self._dummy((g.shape[0], C, H, W), g.device), self._phase_filter(conv),
+                             None, [1, 1], [1, 1], [1, 1], False, [0, 0], 1, [True, False, False])
         return _cl(gi)[0]
 
     def _resnet_f(self, r, x, H, W, tape):
@@ -93,10 +129,8 @@ class DecoderFwdBwd:
         dh = self._conv_b(r.conv2, g, cout, H, W)
         dh = self._gn_b(tape.pop(), dh)
         dh = self._conv_b(r.conv1, dh, cin, H, W)
-        dx = self._gn_b(tape.pop(), dh)
-        if r.conv_shortcut is not None:
-            return ops.add_bias_f32(dx, self._conv_b(r.conv_shortcut, g, cin, H, W))
-        return ops.add_bias_f32(dx, g.contiguous())
+        sc = self._conv_b(r.conv_shortcut, g, cin, H, W) if r.conv_shortcut is not None else g.contiguous()
+        return self._gn_b(tape.pop(), dh, addend=sc)                       # + the shortcut path's gradient
 
     def _attn_f(self, a, x, tape):
         """Single-head self-attention over all tokens (vae._MidAttention), probabilities materialised."""
@@ -143,10 +177,9 @@ class DecoderFwdBwd:
                     x = self._resnet_f(r, x, H, W, tape)
                 if blk.upsamplers is not None:
                     C = x.shape[2]
-                    x = x.view(B, H, 1, W, 1, C).expand(B, H, 2, W, 2, C).reshape(B, 4 * H * W, C)
-                    H, W = 2 * H, 2 * W
-                    x = _conv_f(blk.upsamplers[0].conv, x, H, W)
+                    x = self._upsample_f(blk.upsamplers[0].conv, x, H, W)
                     tape.append(("up", blk.upsamplers[0].conv, H, W, C))
+                    H, W = 2 * H, 2 * W
             x = self._gn_f(d.conv_norm_out, x, True, tape)
             y = _conv_f(d.conv_out, x, H, W)
             tape.append(("out", H, W))
@@ -170,9 +203,7 @@ class DecoderFwdBwd:
             for blk in reversed(d.up_blocks):
                 if blk.upsamplers is not None:
                     _, conv, H, W, C = tape.pop()
-                    g = self._conv_b(conv, g, C, H, W)
-                    H, W = H // 2, W // 2
-                    g = g.view(B, H, 2, W, 2, C).sum(dim=(2, 4)).reshape(B, H * W, C)   # adjoint of nearest x2
+                    g = self._upsample_b(conv, g, H, W, C)
                 for _ in blk.resnets:
                     g = self._resnet_b(tape, g)
             g = self._resnet_b(tape, g)
