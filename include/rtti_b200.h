@@ -72,10 +72,12 @@ int rtti_attn_probs_mean_accum(const void* q, const void* k, const float* lse, f
 /* GroupNorm (+ optional SiLU) over channels-last activations x[batch, hw, c] fp16.
  * Replaces norm1/norm2 + nonlinearity of ResnetBlock2D (models/resnet.py:597-600, 624-629),
  * Transformer2DModel.norm (models/transformer_2d.py:272) and conv_norm_out + conv_act
- * (models/unet_2d_condition.py:975-977).  gamma/beta fp16 [c]; stats in fp32.
+ * (models/unet_2d_condition.py:975-977).  gamma/beta fp16 [c]; stats in fp32. c a multiple of 8 and of groups,
+ * c <= 8192 (RTTI_ERR_SHAPE otherwise).
  *   chan_bias: optional fp16 [batch, c] added to x before the statistics — the time-embedding add
  *   `hidden_states + temb` that precedes norm2 (models/resnet.py:621-622), fused; NULL to skip.
- *   workspace: fp32 [batch * ceil(hw/rows_per_block) * groups * 2] partial sums; query the element
+ *   workspace: fp32 [batch * ceil(hw/rows_per_block) * groups * 2] partial (mean, sum of squared deviations),
+ *   merged pairwise (Chan et al.) so the variance keeps its accuracy for inputs with |mean| >> std; query the element
  *   count with rtti_groupnorm_workspace_elems.  Deterministic (no atomics).
  */
 long long rtti_groupnorm_workspace_elems(int batch, int hw, int c, int groups);
@@ -148,6 +150,7 @@ int rtti_predict_x0(const void* x_t, const void* eps, float alpha, void* x0, lon
 /* fp32 channels-last GroupNorm(+SiLU) forward / input-gradient backward for the VAE decoder that colour guidance
  * differentiates through (third-party AutoencoderKL, called at models/region_diffusion_sdxl.py:856-865 and
  * models/region_diffusion.py:157-165). x, y, dz, dx: [batch, hw, c] fp32; gamma/beta [c] fp32;
+ * c a multiple of 4 and of groups, c <= 2048 (RTTI_ERR_SHAPE otherwise);
  * mean_rstd [batch, groups, 2] fp32 (written by fwd, read by bwd); workspace fp32
  * [rtti_gn32_workspace_elems(...)]. dx = d loss / d x given dz = d loss / d (silu?(GN(x))).
  * chan_bias: optional fp32 [c] added to x first (the bias of the convolution that produced x, folded in); NULL to skip.
@@ -202,7 +205,8 @@ int rtti_gather_blend_step(const void* const* peer_slots, void* const* peer_flag
  *
  * rtti_gn32_silu_fwd/bwd_striped: GroupNorm(+SiLU) over a tensor of hw_total rows of which x holds this rank's
  *   hw_local rows (batch 1, groups <= 32). The statistics are reduced through peer memory inside the call:
- *   peer_sums (host, [world]): device pointers to each rank's fp32 [2 (seq parity)][2*groups] slot;
+ *   peer_sums (host, [world]): device pointers to each rank's fp32 [2 (seq parity)][3*groups] slot (forward: the
+ *   rank's element count, mean and sum of squared deviations per group, merged in rank order; backward: two sums);
  *   peer_flags (host, [world]): device pointers to each rank's uint32[9] {sequence, error, -, ..., [8] sequence base}
  *   words (zero-initialised);
  *   seq: 1, 2, 3, ... the same on every rank for the same call; the kernels add the local rank's sequence base word

@@ -62,8 +62,12 @@ static GNPlan gn_plan(int batch, int hw, int c) {
   return p;
 }
 
-// partial (sum, sumsq) per (batch, chunk, group); fixed summation order.
-__global__ void gn_stats_kernel(const __half* __restrict__ x, const __half* __restrict__ chan_bias,
+// partial (mean, m2) per (batch, chunk, group), m2 = sum of squared deviations from that mean: running (mean, m2) per
+// thread, each batch of 4 rows reduced two-pass in registers and merged in (Chan et al.; Welford's update for the
+// remainder rows), then the (thread, channel) partials merged into the group with stats_merge in a fixed order.
+// No E[x^2] - E[x]^2 cancellation, whatever the offset of x. Up to c/8 = 1024 threads per CTA (rowlanes = 1 once
+// nvec >= 256): the launch bound keeps it within 64 registers, so that every shape the entry point accepts launches.
+__global__ void __launch_bounds__(1024) gn_stats_kernel(const __half* __restrict__ x, const __half* __restrict__ chan_bias,
                                 float* __restrict__ ws, int hw, int c, int groups, int nvec, int rowlanes,
                                 int rows_per_chunk, int chunks) {
   extern __shared__ float sm[];  // [rowlanes][c][2]
@@ -76,29 +80,42 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, const __half* __re
   for (int i = 0; i < 8; ++i) { s[i] = 0.f; ss[i] = 0.f; tb[i] = 0.f; }
   if (chan_bias) unpack8(ld8(chan_bias + (size_t)b * c + vec * 8), tb);
   const __half* base = x + ((size_t)b * hw) * c + vec * 8;
+  int cnt = 0;   // rows seen by this thread; s = running mean, ss = running m2
   int r = r0 + rl;
   for (; r + 3 * rowlanes < r1; r += 4 * rowlanes) {  // 4 independent 128-bit loads in flight per thread
     Half8 v[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) v[u] = ld8(base + (size_t)(r + u * rowlanes) * c);
+    // the 4 rows as one batch (mean, m2), merged into the running statistics: one reciprocal; the halves are
+    // converted a channel pair at a time, which keeps the kernel within 64 registers
+    const float w = 4.f / (float)(cnt + 4), nw = (float)cnt * w;
+    cnt += 4;
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      float f[8];
-      unpack8(v[u], f);
+    for (int j = 0; j < 4; ++j) {
+      float2 t[4];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float t = f[i] + tb[i];
-        s[i] += t; ss[i] += t * t;
+      for (int u = 0; u < 4; ++u) t[u] = __half22float2(v[u].v[j]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int i = 2 * j + h;
+        const float t0 = (h ? t[0].y : t[0].x) + tb[i], t1 = (h ? t[1].y : t[1].x) + tb[i];
+        const float t2 = (h ? t[2].y : t[2].x) + tb[i], t3 = (h ? t[3].y : t[3].x) + tb[i];
+        const float bm = ((t0 + t1) + (t2 + t3)) * 0.25f;
+        const float bq = fmaf(t3 - bm, t3 - bm, fmaf(t2 - bm, t2 - bm, fmaf(t1 - bm, t1 - bm, (t0 - bm) * (t0 - bm))));
+        const float d = bm - s[i];
+        s[i] = fmaf(d, w, s[i]);
+        ss[i] = fmaf(d * d, nw, ss[i] + bq);
       }
     }
   }
   for (; r < r1; r += rowlanes) {
     float f[8];
     unpack8(ld8(base + (size_t)r * c), f);
+    const float rc = 1.f / (float)(++cnt);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
-      const float t = f[i] + tb[i];
-      s[i] += t; ss[i] += t * t;
+      const float t = f[i] + tb[i], d = t - s[i];
+      s[i] = fmaf(d, rc, s[i]); ss[i] = fmaf(d, t - s[i], ss[i]);
     }
   }
 #pragma unroll
@@ -108,36 +125,40 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, const __half* __re
   }
   __syncthreads();
   const int cpg = c / groups;
-  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-    float a = 0.f, q = 0.f;
-    for (int l = 0; l < rowlanes; ++l)
-      for (int ch = g * cpg; ch < (g + 1) * cpg; ++ch) {
-        a += sm[((size_t)l * c + ch) * 2];
-        q += sm[((size_t)l * c + ch) * 2 + 1];
-      }
+  const int nrow = r1 - r0;
+  for (int ch = threadIdx.x; ch < c; ch += blockDim.x) {   // each channel over its row lanes, into row lane 0's slot
+    int n = 0;
+    float mean = 0.f, m2 = 0.f;
+    for (int l = 0; l < rowlanes && l < nrow; ++l)   // row lane l holds ceil((nrow - l) / rowlanes) rows
+      stats_merge(n, mean, m2, (nrow - l + rowlanes - 1) / rowlanes, sm[((size_t)l * c + ch) * 2],
+                  sm[((size_t)l * c + ch) * 2 + 1]);
+    sm[(size_t)ch * 2] = mean; sm[(size_t)ch * 2 + 1] = m2;
+  }
+  __syncthreads();
+  for (int g = threadIdx.x; g < groups; g += blockDim.x) {   // then the group's channels, nrow rows each
+    int n = 0;
+    float mean = 0.f, m2 = 0.f;
+    for (int ch = g * cpg; ch < (g + 1) * cpg; ++ch) stats_merge(n, mean, m2, nrow, sm[(size_t)ch * 2], sm[(size_t)ch * 2 + 1]);
     float* o = ws + (((size_t)b * chunks + chunk) * groups + g) * 2;
-    o[0] = a; o[1] = q;
+    o[0] = mean; o[1] = m2;
   }
 }
 
-// one warp per (batch, group): fixed-order reduction of the chunk partials -> (mean, rstd)
+// one warp per (batch, group): fixed-order Chan merge of the chunk (mean, m2) -> (mean, rstd); chunk k holds
+// min(rows_per_chunk, hw - k*rows_per_chunk) rows of cpg channels
 __global__ void gn_finalize_kernel(const float* __restrict__ ws, float* __restrict__ mean_rstd, int groups, int chunks,
-                                   float n, float eps) {
+                                   int hw, int rows_per_chunk, int cpg, float n, float eps) {
   const int b = blockIdx.y;
   const int g = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (g >= groups) return;
-  float a = 0.f, q = 0.f;
-  for (int k = lane; k < chunks; k += 32) {
-    const float* o = ws + (((size_t)b * chunks + k) * groups + g) * 2;
-    a += o[0]; q += o[1];
-  }
-  a = warp_sum(a); q = warp_sum(q);
+  int cnt;
+  float mean, m2;
+  gn_lane_stats(ws + ((size_t)b * chunks * groups + g) * 2, groups, chunks, hw, rows_per_chunk, cpg, lane, cnt, mean, m2);
+  stats_warp_merge(cnt, mean, m2);
   if (lane == 0) {
-    const float mean = a / n;
-    const float var = fmaxf(q / n - mean * mean, 0.f);
     mean_rstd[((size_t)b * groups + g) * 2] = mean;
-    mean_rstd[((size_t)b * groups + g) * 2 + 1] = rsqrtf(var + eps);
+    mean_rstd[((size_t)b * groups + g) * 2 + 1] = rsqrtf(m2 / n + eps);
   }
 }
 
@@ -509,7 +530,8 @@ extern "C" int rtti_groupnorm_silu_fwd(const void* x, const void* chan_bias, con
   gn_stats_kernel<<<grid, p.threads, sm1, st>>>((const __half*)x, (const __half*)chan_bias, workspace, hw, c, groups,
                                                 p.nvec, p.rowlanes, p.rows_per_chunk, p.chunks);
   float* mean_rstd = workspace + (size_t)batch * p.chunks * groups * 2;
-  gn_finalize_kernel<<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, mean_rstd, groups, p.chunks,
+  gn_finalize_kernel<<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, mean_rstd, groups, p.chunks, hw,
+                                                                    p.rows_per_chunk, c / groups,
                                                                     (float)hw * (float)(c / groups), eps);
   gn_apply_kernel<<<grid, p.threads, 0, st>>>((const __half*)x, (const __half*)chan_bias, (const __half*)gamma,
                                               (const __half*)beta, mean_rstd, (__half*)y, hw, c, groups, p.nvec,

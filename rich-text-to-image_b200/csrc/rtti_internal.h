@@ -19,4 +19,54 @@ int make_head_map(CUtensorMap* m, const void* ptr, int head_dim, int heads, int 
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+#ifdef __CUDACC__
+// GroupNorm statistics of a set of values as (count n, mean, m2 = sum of squared deviations from the mean), merged with
+// the pairwise update of Chan, Golub & LeVeque. Unlike a one-pass E[x^2] - E[x]^2 in fp32, which loses about
+// log10((mean/std)^2) digits of the variance, this keeps the variance as accurate as the inputs whatever their offset.
+// Merging into an empty partial (n = 0) copies the other operand; an empty b is a no-op. The weight nb/(n+nb) uses the
+// fast division (2 ulp): it only scales the correction term, and the merge sits on the serial tail of the reductions.
+__device__ __forceinline__ void stats_merge(int& n, float& mean, float& m2, int nb, float mean_b, float m2_b) {
+  if (nb == 0) return;
+  if (n == 0) { n = nb; mean = mean_b; m2 = m2_b; return; }
+  const int nt = n + nb;
+  const float f = __fdividef((float)nb, (float)nt), d = mean_b - mean;
+  mean = fmaf(d, f, mean);
+  m2 = m2 + m2_b + d * d * ((float)n * f);
+  n = nt;
+}
+
+// (count, mean, m2) of group g over chunks lane, lane+32, ... of a GroupNorm statistics workspace laid out
+// [batch][chunks][groups][2] = (mean, m2); ws_bg points at (b, chunk 0, g). Chunk k holds
+// min(rows_per_chunk, hw - k*rows_per_chunk) rows of cpg channels. The loads of 8 chunks are issued before they are
+// merged (the merge order is still k ascending): the merges form a dependent chain, and one load per merge would put
+// the memory latency on it.
+__device__ __forceinline__ void gn_lane_stats(const float* __restrict__ ws_bg, int groups, int chunks, int hw,
+                                              int rows_per_chunk, int cpg, int lane, int& n, float& mean, float& m2) {
+  n = 0; mean = 0.f; m2 = 0.f;
+  for (int k0 = lane; k0 < chunks; k0 += 32 * 8) {
+    float2 v[8];
+    int nk[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) {
+      const int k = k0 + 32 * u;
+      nk[u] = k < chunks ? min(rows_per_chunk, hw - k * rows_per_chunk) * cpg : 0;
+      v[u] = k < chunks ? *reinterpret_cast<const float2*>(ws_bg + (size_t)k * groups * 2) : make_float2(0.f, 0.f);
+    }
+#pragma unroll
+    for (int u = 0; u < 8; ++u) stats_merge(n, mean, m2, nk[u], v[u].x, v[u].y);
+  }
+}
+
+// fixed-order tree over the 32 lanes of a warp; lane 0 ends with the statistics of every lane
+__device__ __forceinline__ void stats_warp_merge(int& n, float& mean, float& m2) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const int nb = __shfl_down_sync(0xffffffffu, n, o);
+    const float mb = __shfl_down_sync(0xffffffffu, mean, o);
+    const float qb = __shfl_down_sync(0xffffffffu, m2, o);
+    stats_merge(n, mean, m2, nb, mb, qb);
+  }
+}
+#endif
+
 }  // namespace rtti

@@ -3,7 +3,7 @@
 // models/region_diffusion_sdxl.py:856-865; SURVEY §8(f).1).  PyTorch's native GroupNorm copies a
 // channels-last fp32 tensor to NCHW and back and reduces it row-wise (~100 ms of a 350 ms step in the
 // first profile); these kernels work on the NHWC data in place: x [B, HW, C] fp32, groups of C/G channels.
-//   forward : partial (sum, sumsq) per (b, chunk, g)  ->  finalize mean/rstd  ->  y = silu?(xhat*gamma+beta)
+//   forward : partial (mean, m2) per (b, chunk, g)  ->  finalize mean/rstd (Chan merge)  ->  y = silu?(xhat*gamma+beta)
 //   backward: dy = dz * silu'(y) (y recomputed), partial (sum dy*gamma, sum dy*gamma*xhat) -> finalize ->
 //             dx = rstd * (dy*gamma - c1 - xhat*c2)
 // Deterministic (fixed-order two-stage reductions, no atomics); 128-bit vector accesses.
@@ -32,7 +32,11 @@ static GN32Plan gn32_plan(int batch, int hw, int c) {
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }
 
-// MODE 0: (sum x, sum x^2).  MODE 1: backward sums (sum dy*gamma, sum dy*gamma*xhat).
+// MODE 0: (mean, m2) of x per (b, chunk, g), m2 = sum of squared deviations from that mean. Each thread keeps running
+//         (mean, m2) of its rows: each batch of 4 rows is reduced two-pass in registers and merged in (Chan et al.;
+//         Welford's update for the remainder rows), then the (thread, channel) partials are merged into the group with
+//         stats_merge in a fixed order. One read of x, no E[x^2] - E[x]^2 cancellation.
+// MODE 1: backward sums (sum dy*gamma, sum dy*gamma*xhat).
 template <int MODE>
 __global__ void gn32_partial_kernel(const float* __restrict__ x, const float* __restrict__ cbias,
                                     const float* __restrict__ dz,
@@ -61,11 +65,13 @@ __global__ void gn32_partial_kernel(const float* __restrict__ x, const float* __
     }
   }
   const size_t base = ((size_t)b * hw) * c + vec * 4;
+  int cnt = 0;   // MODE 0: rows seen by this thread; a = running mean, q = running m2
   auto accumulate = [&](const float4& xv, const float4& dv) {
     const float xs[4] = {xv.x + cb[0], xv.y + cb[1], xv.z + cb[2], xv.w + cb[3]};
     if (MODE == 0) {
+      const float rc = 1.f / (float)(++cnt);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) { a[i] += xs[i]; q[i] += xs[i] * xs[i]; }
+      for (int i = 0; i < 4; ++i) { const float d = xs[i] - a[i]; a[i] = fmaf(d, rc, a[i]); q[i] = fmaf(d, xs[i] - a[i], q[i]); }
     } else {
       const float ds[4] = {dv.x, dv.y, dv.z, dv.w};
 #pragma unroll
@@ -90,8 +96,26 @@ __global__ void gn32_partial_kernel(const float* __restrict__ x, const float* __
       xv[u] = *reinterpret_cast<const float4*>(x + base + (size_t)(r + u * rowlanes) * c);
       if (MODE == 1) dv[u] = *reinterpret_cast<const float4*>(dz + base + (size_t)(r + u * rowlanes) * c);
     }
+    if (MODE == 0) {   // the 4 rows as one batch (mean, m2), merged into the running statistics: one reciprocal
+      const float w = 4.f / (float)(cnt + 4), nw = (float)cnt * w;
+      cnt += 4;
 #pragma unroll
-    for (int u = 0; u < 4; ++u) accumulate(xv[u], dv[u]);
+      for (int i = 0; i < 4; ++i) {
+        float v[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) v[u] = reinterpret_cast<const float*>(&xv[u])[i] + cb[i];
+        const float bm = ((v[0] + v[1]) + (v[2] + v[3])) * 0.25f;
+        float bq = 0.f;
+#pragma unroll
+        for (int u = 0; u < 4; ++u) bq = fmaf(v[u] - bm, v[u] - bm, bq);
+        const float d = bm - a[i];
+        a[i] = fmaf(d, w, a[i]);
+        q[i] = fmaf(d * d, nw, q[i] + bq);
+      }
+    } else {
+#pragma unroll
+      for (int u = 0; u < 4; ++u) accumulate(xv[u], dv[u]);
+    }
   }
   for (; r < r1; r += rowlanes) {
     const float4 xv = *reinterpret_cast<const float4*>(x + base + (size_t)r * c);
@@ -105,27 +129,55 @@ __global__ void gn32_partial_kernel(const float* __restrict__ x, const float* __
     sm[((size_t)rl * c + vec * 4 + i) * 2 + 1] = q[i];
   }
   __syncthreads();
+  const int nrow = r1 - r0;
+  if (MODE == 0) {   // merge each channel over its row lanes (into row lane 0's slot), all channels in parallel
+    for (int ch = threadIdx.x; ch < c; ch += blockDim.x) {
+      int n = 0;
+      float mean = 0.f, m2 = 0.f;
+      for (int l = 0; l < rowlanes && l < nrow; ++l)   // row lane l holds ceil((nrow - l) / rowlanes) rows
+        stats_merge(n, mean, m2, (nrow - l + rowlanes - 1) / rowlanes, sm[((size_t)l * c + ch) * 2],
+                    sm[((size_t)l * c + ch) * 2 + 1]);
+      sm[(size_t)ch * 2] = mean; sm[(size_t)ch * 2 + 1] = m2;
+    }
+    __syncthreads();
+  }
   for (int g = threadIdx.x; g < groups; g += blockDim.x) {
     float s0 = 0.f, s1 = 0.f;
-    for (int l = 0; l < rowlanes; ++l)
-      for (int ch = g * cpg; ch < (g + 1) * cpg; ++ch) {
-        s0 += sm[((size_t)l * c + ch) * 2];
-        s1 += sm[((size_t)l * c + ch) * 2 + 1];
-      }
+    if (MODE == 0) {   // then the group's channels, nrow rows each
+      int n = 0;
+      for (int ch = g * cpg; ch < (g + 1) * cpg; ++ch) stats_merge(n, s0, s1, nrow, sm[(size_t)ch * 2], sm[(size_t)ch * 2 + 1]);
+    } else {
+      for (int l = 0; l < rowlanes; ++l)
+        for (int ch = g * cpg; ch < (g + 1) * cpg; ++ch) {
+          s0 += sm[((size_t)l * c + ch) * 2];
+          s1 += sm[((size_t)l * c + ch) * 2 + 1];
+        }
+    }
     float* o = ws + (((size_t)b * chunks + chunk) * groups + g) * 2;
     o[0] = s0; o[1] = s1;
   }
 }
 
 // one warp per (b, g): fixed-order reduction of the chunk partials.
-// MODE 0 -> out = (mean, rstd);  MODE 1 -> out = (c1, c2) = sums / n
+// MODE 0 -> out = (mean, rstd) (Chan merge of the chunk (mean, m2));  MODE 1 -> out = (c1, c2) = sums / n
 template <int MODE>
 __global__ void gn32_finalize_kernel(const float* __restrict__ ws, float* __restrict__ out, int groups, int chunks,
-                                     float n, float eps) {
+                                     int hw, int rows_per_chunk, int cpg, float n, float eps) {
   const int b = blockIdx.y;
   const int g = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (g >= groups) return;
+  if (MODE == 0) {
+    int cnt; float mean, m2;
+    gn_lane_stats(ws + ((size_t)b * chunks * groups + g) * 2, groups, chunks, hw, rows_per_chunk, cpg, lane, cnt,
+                    mean, m2);
+    stats_warp_merge(cnt, mean, m2);
+    if (lane == 0) {
+      float* d = out + ((size_t)b * groups + g) * 2;
+      d[0] = mean; d[1] = rsqrtf(m2 / n + eps);
+    }
+    return;
+  }
   float s0 = 0.f, s1 = 0.f;
   for (int k = lane; k < chunks; k += 32) {
     const float* o = ws + (((size_t)b * chunks + k) * groups + g) * 2;
@@ -138,13 +190,7 @@ __global__ void gn32_finalize_kernel(const float* __restrict__ ws, float* __rest
   }
   if (lane == 0) {
     float* d = out + ((size_t)b * groups + g) * 2;
-    if (MODE == 0) {
-      const float mean = s0 / n;
-      const float var = fmaxf(s1 / n - mean * mean, 0.f);
-      d[0] = mean; d[1] = rsqrtf(var + eps);
-    } else {
-      d[0] = s0 / n; d[1] = s1 / n;
-    }
+    d[0] = s0 / n; d[1] = s1 / n;
   }
 }
 
@@ -232,44 +278,53 @@ __global__ void gn32_apply_kernel(const float* __restrict__ x, const float* __re
 static int gn32_check(const void* a, const void* b_, const void* c_, const void* d, int batch, int hw, int c, int groups) {
   if (!a || !b_ || !c_ || !d) return RTTI_ERR_ARG;
   if (batch < 1 || hw < 1 || groups < 1) return RTTI_ERR_ARG;
-  if (c % 4 != 0 || c % groups != 0 || c / 4 > 1024) return RTTI_ERR_SHAPE;
+  // c/4 threads per row lane, so up to c/4 threads per CTA: at most 512, as gn32_partial_kernel<1> and
+  // gn32_apply_kernel<0/1> use 70-82 registers (ptxas, sm_90a) and 1024 x 72+ exceeds the 64K registers of a CTA
+  if (c % 4 != 0 || c % groups != 0 || c / 4 > 512) return RTTI_ERR_SHAPE;
   if (((uintptr_t)a | (uintptr_t)b_ | (uintptr_t)c_ | (uintptr_t)d) & 15) return RTTI_ERR_ALIGN;
   return RTTI_OK;
 }
 
 // ---- stripe-parallel variant (multi-GPU colour guidance, see stripe_exchange.cu) -----------------------------
 struct PeerSums {
-  float* sums[PEER_MAX_WORLD];          // per rank: float [2 parities][2 * groups], peer-mapped
+  float* sums[PEER_MAX_WORLD];          // per rank: float [2 parities][3 * groups], peer-mapped
   unsigned int* flags[PEER_MAX_WORLD];  // per rank: [0] sequence word, [1] error word, [8] sequence base (local rank only)
   int world, rank;
   unsigned int seq;
 };
 
-// One CTA, one warp per group, batch 1: reduce this rank's chunk partials, publish the raw sums, wait for every
-// peer, add the slots in RANK ORDER (bit-identical statistics on all ranks).
+// One CTA, one warp per group, batch 1: reduce this rank's chunk partials, publish them, wait for every peer, merge
+// the slots in RANK ORDER (bit-identical statistics on all ranks). Slot of group g: MODE 0 (count as int bits, mean,
+// m2), merged with stats_merge; MODE 1 (sum, sum, -), added.
 // MODE 0 -> out = (mean, rstd);  MODE 1 -> out = (c1, c2) = sums / n_total
 template <int MODE>
 __global__ void __launch_bounds__(1024) gn32_finalize_peer_kernel(const float* __restrict__ ws, float* __restrict__ out,
-                                                                  const PeerSums pp, int groups, int chunks,
-                                                                  float n_total, float eps) {
+                                                                  const PeerSums pp, int groups, int chunks, int hw,
+                                                                  int rows_per_chunk, int cpg, float n_total,
+                                                                  float eps) {
   const int g = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // effective sequence number = argument + the sequence base word next to this rank's flags (stripe_exchange.cu)
   const unsigned int seq = pp.seq + *reinterpret_cast<const volatile unsigned int*>(pp.flags[pp.rank] + 8);
   const int par = (int)(seq & 1u);
   if (g < groups) {
-    float s0 = 0.f, s1 = 0.f;
-    for (int k = lane; k < chunks; k += 32) {
-      const float* o = ws + ((size_t)k * groups + g) * 2;
-      s0 += o[0]; s1 += o[1];
-    }
+    float* mine = pp.sums[pp.rank] + (size_t)par * 3 * groups + 3 * g;
+    if (MODE == 0) {
+      int cnt; float mean, m2;
+      gn_lane_stats(ws + (size_t)g * 2, groups, chunks, hw, rows_per_chunk, cpg, lane, cnt, mean, m2);
+      stats_warp_merge(cnt, mean, m2);
+      if (lane == 0) { mine[0] = __int_as_float(cnt); mine[1] = mean; mine[2] = m2; }
+    } else {
+      float s0 = 0.f, s1 = 0.f;
+      for (int k = lane; k < chunks; k += 32) {
+        const float* o = ws + ((size_t)k * groups + g) * 2;
+        s0 += o[0]; s1 += o[1];
+      }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      s0 += __shfl_xor_sync(0xffffffffu, s0, o);
-      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-    }
-    if (lane == 0) {
-      float* mine = pp.sums[pp.rank] + (size_t)par * 2 * groups;
-      mine[2 * g] = s0; mine[2 * g + 1] = s1;
+      for (int o = 16; o > 0; o >>= 1) {
+        s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+      }
+      if (lane == 0) { mine[0] = s0; mine[1] = s1; }
     }
   }
   __syncthreads();
@@ -282,18 +337,21 @@ __global__ void __launch_bounds__(1024) gn32_finalize_peer_kernel(const float* _
   }
   __syncthreads();
   if (g < groups && lane == 0) {
-    float t0 = 0.f, t1 = 0.f;
-    for (int r = 0; r < pp.world; ++r) {
-      const float* p = pp.sums[r] + (size_t)par * 2 * groups;
-      t0 += ld_volatile_f32(p + 2 * g);
-      t1 += ld_volatile_f32(p + 2 * g + 1);
-    }
     float* d = out + (size_t)g * 2;
     if (MODE == 0) {
-      const float mean = t0 / n_total;
-      const float var = fmaxf(t1 / n_total - mean * mean, 0.f);
-      d[0] = mean; d[1] = rsqrtf(var + eps);
+      int cnt = 0; float mean = 0.f, m2 = 0.f;
+      for (int r = 0; r < pp.world; ++r) {
+        const float* p = pp.sums[r] + (size_t)par * 3 * groups + 3 * g;
+        stats_merge(cnt, mean, m2, __float_as_int(ld_volatile_f32(p)), ld_volatile_f32(p + 1), ld_volatile_f32(p + 2));
+      }
+      d[0] = mean; d[1] = rsqrtf(m2 / n_total + eps);
     } else {
+      float t0 = 0.f, t1 = 0.f;
+      for (int r = 0; r < pp.world; ++r) {
+        const float* p = pp.sums[r] + (size_t)par * 3 * groups + 3 * g;
+        t0 += ld_volatile_f32(p);
+        t1 += ld_volatile_f32(p + 1);
+      }
       d[0] = t0 / n_total; d[1] = t1 / n_total;
     }
   }
@@ -336,7 +394,8 @@ extern "C" int rtti_gn32_silu_fwd(const float* x, const float* chan_bias, const 
   dim3 grid(p.chunks, batch);
   gn32_partial_kernel<0><<<grid, p.threads, smem, st>>>(x, chan_bias, nullptr, gamma, beta, nullptr, workspace, hw, c, groups,
                                                         p.nvec, p.rowlanes, p.rows_per_chunk, p.chunks, 0);
-  gn32_finalize_kernel<0><<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, mean_rstd, groups, p.chunks,
+  gn32_finalize_kernel<0><<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, mean_rstd, groups, p.chunks, hw,
+                                                                         p.rows_per_chunk, c / groups,
                                                                          (float)hw * (float)(c / groups), eps);
   gn32_apply_kernel<0><<<grid, p.threads, 0, st>>>(x, chan_bias, nullptr, gamma, beta, mean_rstd, nullptr, nullptr, y, hw, c,
                                                    groups, p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
@@ -358,7 +417,8 @@ extern "C" int rtti_gn32_silu_bwd(const float* x, const float* chan_bias, const 
   float* c12 = workspace + (size_t)batch * p.chunks * groups * 2;
   gn32_partial_kernel<1><<<grid, p.threads, smem, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, workspace, hw, c, groups, p.nvec,
                                                         p.rowlanes, p.rows_per_chunk, p.chunks, apply_silu);
-  gn32_finalize_kernel<1><<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, c12, groups, p.chunks,
+  gn32_finalize_kernel<1><<<dim3((groups + 7) / 8, batch), 256, 0, st>>>(workspace, c12, groups, p.chunks, hw,
+                                                                         p.rows_per_chunk, c / groups,
                                                                          (float)hw * (float)(c / groups), 0.f);
   gn32_apply_kernel<1><<<grid, p.threads, 0, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, c12, addend, dx, hw, c, groups,
                                                    p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
@@ -384,7 +444,8 @@ extern "C" int rtti_gn32_silu_fwd_striped(const float* x, const float* chan_bias
   dim3 grid(p.chunks, 1);
   gn32_partial_kernel<0><<<grid, p.threads, smem, st>>>(x, chan_bias, nullptr, gamma, beta, nullptr, workspace, hw_local, c,
                                                         groups, p.nvec, p.rowlanes, p.rows_per_chunk, p.chunks, 0);
-  gn32_finalize_peer_kernel<0><<<1, 32 * groups, 0, st>>>(workspace, mean_rstd, pp, groups, p.chunks,
+  gn32_finalize_peer_kernel<0><<<1, 32 * groups, 0, st>>>(workspace, mean_rstd, pp, groups, p.chunks, hw_local,
+                                                          p.rows_per_chunk, c / groups,
                                                           (float)hw_total * (float)(c / groups), eps);
   gn32_apply_kernel<0><<<grid, p.threads, 0, st>>>(x, chan_bias, nullptr, gamma, beta, mean_rstd, nullptr, nullptr, y, hw_local,
                                                    c, groups, p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);
@@ -411,7 +472,8 @@ extern "C" int rtti_gn32_silu_bwd_striped(const float* x, const float* chan_bias
   float* c12 = workspace + (size_t)p.chunks * groups * 2;
   gn32_partial_kernel<1><<<grid, p.threads, smem, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, workspace, hw_local, c,
                                                         groups, p.nvec, p.rowlanes, p.rows_per_chunk, p.chunks, apply_silu);
-  gn32_finalize_peer_kernel<1><<<1, 32 * groups, 0, st>>>(workspace, c12, pp, groups, p.chunks,
+  gn32_finalize_peer_kernel<1><<<1, 32 * groups, 0, st>>>(workspace, c12, pp, groups, p.chunks, hw_local,
+                                                          p.rows_per_chunk, c / groups,
                                                           (float)hw_total * (float)(c / groups), 0.f);
   gn32_apply_kernel<1><<<grid, p.threads, 0, st>>>(x, chan_bias, dz, gamma, beta, mean_rstd, c12, nullptr, dx, hw_local, c,
                                                    groups, p.nvec, p.rowlanes, p.rows_per_chunk, apply_silu);

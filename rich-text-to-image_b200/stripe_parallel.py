@@ -43,7 +43,7 @@ class StripeArena:
     """Symmetric arena: [4 KB control block][pad half 0][pad half 1], identical layout on every rank.
 
     Control block: +0 GroupNorm {sequence, error, ..., [8] sequence base} words; +64 halo flags {from_up, from_down,
-    error, counter, ..., [8] sequence base}; +256 GroupNorm sum slots fp32 [2 parities][2 * 32 groups]. Pads alternate
+    error, counter, ..., [8] sequence base}; +256 GroupNorm statistics slots fp32 [2 parities][3 * 32 groups]. Pads alternate
     between the two halves by exchange sequence parity (see csrc/stripe_exchange.cu for why two are enough).
 
     Sequence numbers are RELATIVE to one decoder evaluation (forward + backward): the host counts 1..n, the kernels add

@@ -37,10 +37,14 @@ def fake_ops(reduce_over_ranks):
     """name -> emulation. reduce_over_ranks(key, tensor) returns the sum of `tensor` over the ranks (the peer
     reduction of gn32_finalize_peer_kernel); every rank must call it in the same order."""
     def gn_stats(x, cb, groups, n, eps, red):
+        # per rank (count, mean, sum of squared deviations) merged over the ranks (Chan et al.), as the kernels do
         xs = x[0] + (cb if cb is not None else 0)
-        s0, s1 = red(_group_sums(xs, groups)), red(_group_sums(xs * xs, groups))
-        mean = s0 / n
-        rstd = torch.rsqrt((s1 / n - mean * mean).clamp_min(0) + eps)
+        n_r = xs.numel() // groups
+        mean_r = _group_sums(xs, groups) / n_r
+        m2_r = _group_sums((xs - mean_r.repeat_interleave(xs.shape[1] // groups)) ** 2, groups)
+        mean = red(mean_r * n_r) / n
+        m2 = red(m2_r + n_r * (mean_r - mean) ** 2)
+        rstd = torch.rsqrt(m2 / n + eps)
         return xs, torch.stack([mean, rstd], 1)[None]
 
     def gn_fwd(x, gamma, beta, groups, eps, silu, n, red, chan_bias, out):
