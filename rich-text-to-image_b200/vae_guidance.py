@@ -16,7 +16,12 @@ static sequence — no autograd graph, no autograd thread, CUDA-graph capturable
     high-res tensor (and the gradient scattered back) by csrc/vae_kernels.cu;
   * the single-head 16384-token mid-block attention materialises its 1 GB probability matrix once
     and reuses it for the five backward GEMMs instead of recomputing it.
+
+DecoderFwdBwd.forward / .backward are the one walk over the decoder's blocks. They hand the engine's activation from
+layer to layer: here a [B, H*W, C] tensor; in the stripe-parallel engine, which overrides the per-layer methods
+(stripe_parallel.py says which), this rank's stripe of rows.
 """
+import contextlib
 import math
 
 import torch
@@ -32,8 +37,15 @@ _conv_bwd = torch.ops.aten.convolution_backward
 _PHASE_TAPS = (((1., 0., 0.), (0., 1., 1.)), ((1., 1., 0.), (0., 0., 1.)))
 
 
-class _Tape(list):
-    pass
+@contextlib.contextmanager
+def _tf32_matmul():
+    """fp32 matmuls (projections, attention) on TF32 tensor cores; the caller's setting is restored on exit."""
+    prev = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = True
+    try:
+        yield
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev
 
 
 def _nchw(x, H, W):
@@ -132,43 +144,73 @@ class DecoderFwdBwd:
         sc = self._conv_b(r.conv_shortcut, g, cin, H, W) if r.conv_shortcut is not None else g.contiguous()
         return self._gn_b(tape.pop(), dh, addend=sc)                       # + the shortcut path's gradient
 
+    def _attn_kv(self, hn):
+        """Normalised tokens the keys and values are projected from."""
+        return hn
+
+    def _attn_dhn(self, a, dq, dk, dv):
+        """Gradient of the attention's normalised input from those of q, k, v."""
+        return dq @ a.to_q.weight + dk @ a.to_k.weight + dv @ a.to_v.weight
+
     def _attn_f(self, a, x, tape):
         """Single-head self-attention over all tokens (vae._MidAttention), probabilities materialised."""
-        B, T, C = x.shape
+        C = x.shape[2]
         hn = self._gn_f(a.group_norm, x, False, tape)
+        kv = self._attn_kv(hn)
         q = F.linear(hn, a.to_q.weight, a.to_q.bias)
-        k = F.linear(hn, a.to_k.weight, a.to_k.bias)
-        v = F.linear(hn, a.to_v.weight, a.to_v.bias)
+        k = F.linear(kv, a.to_k.weight, a.to_k.bias)
+        v = F.linear(kv, a.to_v.weight, a.to_v.bias)
         scale = 1.0 / math.sqrt(C)
         # the softmax scale is applied to q ([T, C], 33 MB) instead of the [T, T] scores (1 GB at 1024^2: a 2 GB pass)
         p = torch.softmax(torch.bmm(q * scale, k.transpose(1, 2)), dim=-1)
         o = torch.bmm(p, v)
-        tape.append(("attn", a, hn, q, k, v, p, scale))
+        tape.append(("attn", a, q, k, v, p, scale))
         return x + F.linear(o, a.to_out[0].weight, a.to_out[0].bias)
 
     def _attn_b(self, tape, g):
-        _, a, hn, q, k, v, p, scale = tape.pop()
+        _, a, q, k, v, p, scale = tape.pop()
         do = g @ a.to_out[0].weight                       # [B,T,C]
         dv = torch.bmm(p.transpose(1, 2), do)
         dp = torch.bmm(do, v.transpose(1, 2))
         ds = torch._softmax_backward_data(dp, p, -1, p.dtype)   # d/d(scaled scores); the scale goes onto the small operands
         dq = torch.bmm(ds, k * scale)
         dk = torch.bmm(ds.transpose(1, 2), q * scale)
-        dhn = dq @ a.to_q.weight + dk @ a.to_k.weight + dv @ a.to_v.weight
-        return g + self._gn_b(tape.pop(), dhn)
+        return g + self._gn_b(tape.pop(), self._attn_dhn(a, dq, dk, dv))
+
+    def _entry(self, z):
+        """z [B, 4, H, W] -> (activation after conv_in, H, W)."""
+        vae, d = self.vae, self.vae.decoder
+        B, _, H, W = z.shape
+        x = z.permute(0, 2, 3, 1).contiguous().view(B, H * W, -1)
+        x = _conv_f(vae.post_quant_conv, x, H, W)
+        return _conv_f(d.conv_in, x, H, W), H, W
+
+    def _out_f(self, x, H, W, tape):
+        """conv_norm_out + SiLU + conv_out -> image [B, 3, H, W] (NCHW view of channels-last memory)."""
+        d = self.vae.decoder
+        x = self._gn_f(d.conv_norm_out, x, True, tape)
+        return _nchw(_conv_f(d.conv_out, x, H, W), H, W)
+
+    def _out_b(self, grad_image, H, W, tape):
+        d = self.vae.decoder
+        g = grad_image.permute(0, 2, 3, 1).contiguous().view(grad_image.shape[0], H * W, -1)
+        g = self._conv_b(d.conv_out, g, d.conv_out.in_channels, H, W)
+        return self._gn_b(tape.pop(), g)
+
+    def _exit(self, g, H, W):
+        """Gradient after conv_in's output -> d z [B, 4, H, W]."""
+        vae, d = self.vae, self.vae.decoder
+        g = self._conv_b(d.conv_in, g, d.conv_in.in_channels, H, W)
+        g = self._conv_b(vae.post_quant_conv, g, vae.post_quant_conv.in_channels, H, W)
+        return g.view(g.shape[0], H, W, -1).permute(0, 3, 1, 2).contiguous()
 
     # ------------------------------------------------------------------ whole decoder
     def forward(self, z):
         """z [B, 4, h, w] fp32 -> image [B, 3, 8h, 8w] fp32 (NCHW view of channels-last memory); keeps the tape."""
-        vae, d = self.vae, self.vae.decoder
-        prev = torch.backends.cuda.matmul.allow_tf32
-        torch.backends.cuda.matmul.allow_tf32 = True
-        try:
-            tape = _Tape()
-            B, _, H, W = z.shape
-            x = z.permute(0, 2, 3, 1).contiguous().view(B, H * W, -1)
-            x = _conv_f(vae.post_quant_conv, x, H, W)
-            x = _conv_f(d.conv_in, x, H, W)
+        d = self.vae.decoder
+        with _tf32_matmul():
+            tape = []
+            x, H, W = self._entry(z)
             x = self._resnet_f(d.mid_block.resnets[0], x, H, W, tape)
             x = self._attn_f(d.mid_block.attentions[0], x, tape)
             x = self._resnet_f(d.mid_block.resnets[1], x, H, W, tape)
@@ -176,30 +218,22 @@ class DecoderFwdBwd:
                 for r in blk.resnets:
                     x = self._resnet_f(r, x, H, W, tape)
                 if blk.upsamplers is not None:
-                    C = x.shape[2]
-                    x = self._upsample_f(blk.upsamplers[0].conv, x, H, W)
-                    tape.append(("up", blk.upsamplers[0].conv, H, W, C))
+                    conv, C = blk.upsamplers[0].conv, x.shape[2]
+                    x = self._upsample_f(conv, x, H, W)
+                    tape.append(("up", conv, H, W, C))
                     H, W = 2 * H, 2 * W
-            x = self._gn_f(d.conv_norm_out, x, True, tape)
-            y = _conv_f(d.conv_out, x, H, W)
+            img = self._out_f(x, H, W, tape)
             tape.append(("out", H, W))
             self.tape = tape
-            return _nchw(y, H, W)
-        finally:
-            torch.backends.cuda.matmul.allow_tf32 = prev
+            return img
 
     def backward(self, grad_image):
         """grad_image [B, 3, H, W] -> d loss / d z [B, 4, h, w] fp32."""
-        vae, d = self.vae, self.vae.decoder
-        prev = torch.backends.cuda.matmul.allow_tf32
-        torch.backends.cuda.matmul.allow_tf32 = True
-        try:
+        d = self.vae.decoder
+        with _tf32_matmul():
             tape = self.tape
             _, H, W = tape.pop()
-            B = grad_image.shape[0]
-            g = grad_image.permute(0, 2, 3, 1).contiguous().view(B, H * W, -1)
-            g = self._conv_b(d.conv_out, g, d.conv_out.in_channels, H, W)
-            g = self._gn_b(tape.pop(), g)
+            g = self._out_b(grad_image, H, W, tape)
             for blk in reversed(d.up_blocks):
                 if blk.upsamplers is not None:
                     _, conv, H, W, C = tape.pop()
@@ -209,12 +243,8 @@ class DecoderFwdBwd:
             g = self._resnet_b(tape, g)
             g = self._attn_b(tape, g)
             g = self._resnet_b(tape, g)
-            g = self._conv_b(d.conv_in, g, d.conv_in.in_channels, H, W)
-            g = self._conv_b(vae.post_quant_conv, g, vae.post_quant_conv.in_channels, H, W)
             self.tape = None
-            return g.view(B, H, W, -1).permute(0, 3, 1, 2).contiguous()
-        finally:
-            torch.backends.cuda.matmul.allow_tf32 = prev
+            return self._exit(g, H, W)
 
 
 def default_engine(vae):

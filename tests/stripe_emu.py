@@ -1,6 +1,7 @@
-"""Torch emulations of the stripe-parallel kernels' C-ABI contracts (include/rtti_b200.h: rtti_gn32_silu_fwd/bwd,
-rtti_gn32_silu_*_striped, rtti_add_bias_f32) for the CPU tests of rtti_b200/stripe_parallel.py. Test infrastructure
-only: the product path never imports this module."""
+"""Torch emulations of the colour-guidance decoder kernels' C-ABI contracts (include/rtti_b200.h: rtti_gn32_silu_fwd/bwd,
+rtti_gn32_silu_*_striped, rtti_add_bias_f32, rtti_upsample_phase_interleave/_scatter) for the CPU tests of
+rtti_b200/vae_guidance.py and rtti_b200/stripe_parallel.py. Test infrastructure only: the product path never imports
+this module."""
 import torch
 import torch.nn.functional as F
 
@@ -82,11 +83,14 @@ def fake_ops(reduce_over_ranks):
         r = a + b + (bias if bias is not None else 0)
         return r if out is None else out.copy_(r)
 
+    def gn_bwd_addend(x, dz, g, b, stats, groups, silu, chan_bias=None, addend=None):
+        dx = gn_bwd(x, dz, g, b, stats, groups, silu, x.shape[1] * x.shape[2] // groups, ident, chan_bias, None)
+        return dx if addend is None else dx + addend
+
     return {
         "gn32_silu_fwd": lambda x, g, b, groups, eps, silu, chan_bias=None:
             gn_fwd(x, g, b, groups, eps, silu, x.shape[1] * x.shape[2] // groups, ident, chan_bias, None),
-        "gn32_silu_bwd": lambda x, dz, g, b, stats, groups, silu, chan_bias=None:
-            gn_bwd(x, dz, g, b, stats, groups, silu, x.shape[1] * x.shape[2] // groups, ident, chan_bias, None),
+        "gn32_silu_bwd": gn_bwd_addend,
         "gn32_silu_fwd_striped": lambda x, g, b, groups, eps, silu, hw_total, peers, seq, chan_bias=None, out=None:
             gn_fwd(x, g, b, groups, eps, silu, hw_total * x.shape[2] // groups,
                    lambda v: reduce_over_ranks(("gn", seq), v), chan_bias, out),
@@ -94,7 +98,32 @@ def fake_ops(reduce_over_ranks):
             gn_bwd(x, dz, g, b, stats, groups, silu, hw_total * x.shape[2] // groups,
                    lambda v: reduce_over_ranks(("gn", seq), v), chan_bias, out),
         "add_bias_f32": add_bias,
+        "upsample_phase_interleave": upsample_phase_interleave,
+        "upsample_phase_scatter": upsample_phase_scatter,
     }
+
+
+def upsample_phase_interleave(y4, bias, h, w):
+    """y4 [B, (h+1)*(w+1), 4C], phase 2a+b in channels (2a+b)*C.. -> [B, 4*h*w, C]: output pixel (2i+a, 2j+b) is
+    phase (a, b) of low-res position (i+a, j+b), plus bias."""
+    B, C = y4.shape[0], y4.shape[2] // 4
+    t = y4.view(B, h + 1, w + 1, 2, 2, C)
+    out = torch.empty(B, 2 * h, 2 * w, C, dtype=y4.dtype)
+    for a in range(2):
+        for b in range(2):
+            out[:, a::2, b::2] = t[:, a:a + h, b:b + w, a, b] + (bias if bias is not None else 0)
+    return out.view(B, 4 * h * w, C)
+
+
+def upsample_phase_scatter(g, h, w):
+    """Adjoint of upsample_phase_interleave: g [B, 4*h*w, C] -> [B, (h+1)*(w+1), 4C], zero where no pixel maps."""
+    B, C = g.shape[0], g.shape[2]
+    g5 = g.view(B, 2 * h, 2 * w, C)
+    d4 = g.new_zeros(B, h + 1, w + 1, 2, 2, C)
+    for a in range(2):
+        for b in range(2):
+            d4[:, a:a + h, b:b + w, a, b] = g5[:, a::2, b::2]
+    return d4.view(B, (h + 1) * (w + 1), 4 * C)
 
 
 class FakeArenaBase:

@@ -5,14 +5,34 @@ include/rtti_b200.h (tests/stripe_emu.py), the ranks are threads, and the collec
 the orchestration the GPU cannot check cheaply: stripe bookkeeping and tape order, halo rows, the flipped-filter data
 gradient, global GroupNorm statistics, in-place pad re-use by parity — against plain autograd through the same
 decoder. The same engine runs over real torch.distributed (gloo) in tests/test_distributed_cpu.py; the kernels
-themselves are covered by tests/multigpu_check.py on GPUs."""
+themselves are covered by tests/multigpu_check.py on GPUs. The single-GPU engine, whose decoder walk the striped
+engine shares, runs on the same emulations."""
 import threading
 
 import pytest
 import torch
 
-from rtti_b200 import ops, stripe_parallel
+from rtti_b200 import ops, stripe_parallel, vae_guidance
 from tests import stripe_emu
+
+
+def test_single_gpu_decoder_matches_autograd(monkeypatch):
+    """vae_guidance.DecoderFwdBwd (phase-folded upsamplers, GroupNorm backward with the shortcut gradient as addend)
+    over two calls against autograd through the same decoder."""
+    torch.manual_seed(0)
+    vae = stripe_emu.make_vae()
+    for name, fn in stripe_emu.fake_ops(lambda key, v: v).items():
+        monkeypatch.setattr(ops, name, fn)
+    zs = [torch.randn(1, 4, 8, 8) for _ in range(2)]
+    wgt = torch.randn(1, 3, 64, 64)
+    grad_fn = lambda img: torch.tanh(img) * wgt
+    want = stripe_emu.autograd_reference(vae, zs, grad_fn)
+    eng = vae_guidance.DecoderFwdBwd(vae)
+    res = []
+    for z in zs:
+        img = eng.forward(z)
+        res.append((img.clone(), eng.backward(grad_fn(img))))
+    stripe_emu.assert_matches(res, want)
 
 
 class _World:
@@ -187,7 +207,7 @@ class _AsyncArena(stripe_emu.FakeArenaBase):
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_striped_decoder_async_protocol(monkeypatch, seed):
     """World 4 without lock-step: exercises the claim that two pad halves / two sum slots, alternating by sequence
-    parity, are enough (csrc/stripe_exchange.cu header, stripe_parallel._s_resnet_b docstring)."""
+    parity, are enough (csrc/stripe_exchange.cu header, StripedDecoderFwdBwd._resnet_b docstring)."""
     world = 4
     torch.manual_seed(0)
     torch.set_num_threads(1)
