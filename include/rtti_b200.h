@@ -250,6 +250,30 @@ int rtti_peer_push(const void* src, long long src_row_stride_bytes, int rows, in
                    void* const* dst_flags, int n_dst, void* flags_local, unsigned int seq, void* stream);
 int rtti_peer_wait(void* flags_local, unsigned int seq, void* stream);
 
+/* k-means of the spectral embedding of the token-map affinity: the KMeans(n_clusters, n_init) that scikit-learn's
+ * SpectralClustering(affinity="precomputed", assign_labels="kmeans") runs (utils/attention_utils.py:262-265), all
+ * restarts in one launch (one CTA each). Each restart is k-means++ seeding followed by Lloyd iterations, step for step
+ * as scikit-learn's dense KMeans.fit: centring on the column means, n_local_trials = 2 + floor(ln k), candidates drawn
+ * from the float32 cumulative sum of the float64-formed squared distances (searchsorted side='left', clipped to n-1),
+ * the candidate of lowest potential kept (first on a tie); nearest centre by ||c||^2 - 2 x.c (first on a tie), empty
+ * clusters relocated to the farthest samples, stop when the labels repeat, when the summed squared centre shift is
+ * <= tol * mean(var(x, axis=0)), or after max_iter, then a final assignment unless the labels repeated.
+ *   x [n, k] fp32 row-major; 1 <= k <= 32, k <= n <= 4096 and 4*n*(k+2) + 18 KB <= 227 KB of shared memory
+ *   (n = 4096 allows k <= 11; RTTI_ERR_SHAPE otherwise).
+ *   draws [n_init, 1 + (k-1)*(2 + floor(ln k))] fp64: per restart the index of the first centre, then the uniforms
+ *   in [0, 1) of the k-1 k-means++ steps, as scikit-learn takes them from its RandomState.
+ *   labels [n_init, n] int32, inertia [n_init] fp64 (sum of squared distances to the assigned centres), n_iter [n_init]
+ *   int32: per restart. Choosing among restarts is left to the caller.
+ *   flags [n_init] int32: bit 0 set when the restart relocated empty clusters in a step where scikit-learn's choice is
+ *   left to np.argpartition's unspecified order (two or more clusters empty at once, or distinct samples tied at the
+ *   largest distance); that restart's labels may then differ from scikit-learn's by a renaming.
+ *   n_init >= 1, max_iter >= 1, tol >= 0 (RTTI_ERR_ARG otherwise). Deterministic (no atomics).
+ * rtti_kmeans_supported: host-only query, RTTI_OK when rtti_kmeans_fit accepts (n, k), RTTI_ERR_SHAPE otherwise.
+ */
+int rtti_kmeans_fit(const float* x, const double* draws, int n, int k, int n_init, int max_iter, double tol,
+                    int* labels, double* inertia, int* n_iter, int* flags, void* stream);
+int rtti_kmeans_supported(int n, int k);
+
 #ifdef __cplusplus
 }
 #endif

@@ -62,6 +62,8 @@ SIGNATURES = {
     "rtti_peer_push": (c_int, [c_void_p, c_ll, c_int, c_int, ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int,
                                c_void_p, ctypes.c_uint, c_void_p]),
     "rtti_peer_wait": (c_int, [c_void_p, ctypes.c_uint, c_void_p]),
+    "rtti_kmeans_fit": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [ctypes.c_double] + [c_void_p] * 5),
+    "rtti_kmeans_supported": (c_int, [c_int, c_int]),
 }
 
 _lib = None

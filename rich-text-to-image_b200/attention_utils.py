@@ -1,10 +1,13 @@
 """Token maps: layer allow-lists and get_token_maps (drop-in for utils/attention_utils.py:12-67, 233-341).
 
 The captured maps arrive as fp32 DEVICE tensors (unet.TokenMapAccumulator) instead of fp16 CPU tensors:
-averaging and the bicubic resizes run on the GPU; the spectral clustering stays the reference's own
-scikit-learn call on the host (utils/attention_utils.py:262-265) so the segment labels are the ones the
-reference would produce for the same affinity (SURVEY §8(f).3 lists a GPU eigensolver as "next").
-The debug JPEG / matplotlib dumps of the reference are not reproduced.
+averaging and the bicubic resizes run on the GPU, and so does the spectral clustering of the affinity
+(utils/attention_utils.py:262-265): `spectral_clustering` takes the spectral embedding from a float64 `eigh` of the
+normalised Laplacian and runs the 100 k-means restarts in one kernel (rtti_kmeans_fit), with the random draws taken
+from NumPy's global RandomState exactly as scikit-learn takes them, so the segment labels are the ones scikit-learn's
+SpectralClustering gives for the same affinity. Affinities whose k-th eigenvalue is not separated from the next one
+are handed to scikit-learn (see EIGENGAP_MIN). Maps on the CPU (the reference's fp16 host maps) keep the
+scikit-learn call. The debug JPEG / matplotlib dumps of the reference are not reproduced.
 """
 import random
 
@@ -83,19 +86,111 @@ def render_token_maps(resized):
     return np.concatenate(tiles, axis=1)
 
 
+# Smallest eigengap lambda_{k+1} - lambda_k of the normalised Laplacian for which spectral_clustering runs on the
+# device. Below it the k-th eigenvector is only defined up to rounding: scikit-learn's own float32 ARPACK embedding,
+# and with it its labels, are then decided by rounding noise that a different eigensolver cannot reproduce. With the
+# guard disabled, eigh + the restated kernel gave scikit-learn's labels and RNG state at gaps of 3.8e-7, 1.0e-6, 2.0e-6
+# and 3.9e-6 (near-uniform affinities, k = 4; GAP_SWEEP in tests/test_token_map_clustering.py), 3.9e-6 to 1.3e-5
+# (synth_maps, k = 9) and 2.5e-4 and up (soft blobs). Near-uniform affinities at k = 9 with gaps of 1.2e-11 and 4.9e-12 gave different labels. The threshold
+# keeps the device path to gaps that were shown to match, with the smallest matching gap (3.8e-7) below it.
+EIGENGAP_MIN = 1e-6
+
+
+def kmeans_draws(rs, n, k, n_init):
+    """The random numbers KMeans(k, n_init=n_init).fit takes from RandomState `rs` for n samples of unit weight, in the
+    order it takes them, as [n_init, 1 + (k-1)*trials] float64: per restart the index of the first centre
+    (`rs.choice(n, p=w)`) and then the k-1 `rs.uniform(size=trials)` draws of k-means++
+    (sklearn/cluster/_kmeans.py:_kmeans_plusplus). Leaves `rs` in the state KMeans leaves it in."""
+    trials = 2 + int(np.log(k))
+    u = rs.random_sample(n_init * (1 + (k - 1) * trials)).reshape(n_init, -1)
+    p = np.ones(n, np.float32)
+    cdf = (p / p.sum()).astype(np.float64).cumsum()     # RandomState.choice(n, p=...)
+    cdf /= cdf[-1]
+    u[:, 0] = cdf.searchsorted(u[:, 0], side="right")
+    return u
+
+
+def spectral_embedding(affinity, k):
+    """[n, k] float32 embedding that scikit-learn's SpectralClustering feeds to k-means, up to a rotation inside each
+    eigenspace (which k-means++ and Lloyd do not see), and the eigenvalues of the normalised Laplacian (float64).
+    Same construction as sklearn.manifold.spectral_embedding with drop_first=False: S = (A + A^T)/2, degrees without
+    the self-loops (zero degrees count as 1), L = I - D^-1/2 S D^-1/2 with unit diagonal, the k eigenvectors of the
+    smallest eigenvalues divided by sqrt(degree)."""
+    a = affinity.to(torch.float64)
+    s = 0.5 * (a + a.T)
+    deg = s.sum(1) - s.diagonal()
+    deg = torch.where(deg == 0, torch.ones_like(deg), deg)
+    dh = deg.sqrt()
+    lap = -s / dh[:, None] / dh[None, :]
+    lap.diagonal().fill_(1.0)
+    evals, evecs = torch.linalg.eigh(lap)
+    return (evecs[:, :k] / dh[:, None]).to(torch.float32), evals
+
+
+def select_restart(labels, inertia, k):
+    """KMeans.fit's choice among restarts: a restart replaces the best so far only when its inertia is strictly lower
+    and its labels are not the same clustering up to a renaming."""
+    def same(a, b):   # sklearn's _is_same_clustering: every label of a maps to one label of b
+        return len(np.unique(a.astype(np.int64) * k + b)) == len(np.unique(a))
+    best = 0
+    for r in range(1, len(inertia)):
+        if inertia[r] < inertia[best] and not same(labels[r], labels[best]):
+            best = r
+    return best
+
+
+def _sklearn_spectral(affinity, n_clusters, n_init):
+    from sklearn.cluster import SpectralClustering
+    sc = SpectralClustering(n_clusters, affinity="precomputed", n_init=n_init, assign_labels="kmeans")
+    return sc.fit_predict(affinity.cpu().numpy()).astype(np.int32)
+
+
+def spectral_clustering(affinity, n_clusters, n_init=100, kmeans_fit=None):
+    """Drop-in for SpectralClustering(n_clusters, affinity="precomputed", n_init=n_init, assign_labels="kmeans")
+    .fit_predict(affinity) on NumPy's global RandomState: the same int32 labels [n], and np.random left in the same
+    state. affinity: [n, n] float32 tensor (CUDA for the kernel path). kmeans_fit defaults to rtti_b200.ops.kmeans_fit
+    (the tests substitute a NumPy restatement).
+    The affinity is handed to scikit-learn instead when the kernel does not take the shape (k > 32, n > 4096, ...),
+    when the eigengap lambda_{k+1} - lambda_k is below EIGENGAP_MIN, or when a restart relocated empty clusters in an
+    order scikit-learn leaves unspecified (the RNG is rewound first)."""
+    from . import ops
+    n = affinity.shape[0]
+    if not ops.kmeans_supported(n, n_clusters):
+        return _sklearn_spectral(affinity, n_clusters, n_init)
+    emb, evals = spectral_embedding(affinity, n_clusters)
+    if n_clusters < n and float(evals[n_clusters] - evals[n_clusters - 1]) < EIGENGAP_MIN:
+        return _sklearn_spectral(affinity, n_clusters, n_init)
+    rs = np.random.mtrand._rand
+    state = rs.get_state()
+    rs.uniform(-1, 1, n)   # the ARPACK start vector (sklearn.utils._arpack._init_arpack_v0)
+    draws = kmeans_draws(rs, n, n_clusters, n_init)
+    if kmeans_fit is None:
+        kmeans_fit = ops.kmeans_fit
+        draws = torch.from_numpy(draws).to(emb.device)
+    labels, inertia, _, flags = (np.asarray(v.cpu()) if torch.is_tensor(v) else np.asarray(v)
+                                 for v in kmeans_fit(emb, draws))
+    if flags.any():
+        rs.set_state(state)
+        return _sklearn_spectral(affinity, n_clusters, n_init)
+    return labels[select_restart(labels, inertia, n_clusters)].astype(np.int32)
+
+
 def get_token_maps(selfattn_maps, crossattn_maps, n_maps, save_dir, width, height, obj_tokens, seed=0,
                    tokens_vis=None, preprocess=False, segment_threshold=0.3, num_segments=5, return_vis=False,
                    save_attn=False, device=None, return_clusters=False):
     """Same signature and return value as utils/attention_utils.py:233-341: a list of N masks
     [1, 4, height, width] fp32 (spans..., background) that sum to one per pixel."""
-    from sklearn.cluster import SpectralClustering
     resolution = 32
     some = next(iter(selfattn_maps.values()))
     device = device or some.device
-    aff = self_affinity(selfattn_maps, resolution).cpu().numpy()
+    aff = self_affinity(selfattn_maps, resolution)
     seed_everything(seed)
-    sc = SpectralClustering(num_segments, affinity="precomputed", n_init=100, assign_labels="kmeans")
-    clusters = sc.fit_predict(aff).reshape(resolution, resolution)
+    if aff.is_cuda:
+        clusters = spectral_clustering(aff, num_segments).reshape(resolution, resolution)
+    else:   # the reference's fp16 host maps: scikit-learn, the only path on the CPU
+        from sklearn.cluster import SpectralClustering
+        sc = SpectralClustering(num_segments, affinity="precomputed", n_init=100, assign_labels="kmeans")
+        clusters = sc.fit_predict(aff.numpy()).reshape(resolution, resolution)
     cross = cross_maps_mean(crossattn_maps, resolution).cpu().numpy()
 
     normalized_span_maps = []

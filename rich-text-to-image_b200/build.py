@@ -12,7 +12,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 BUILD_DIR = os.path.join(PKG_DIR, "build")
 LIB_PATH = os.path.join(PKG_DIR, "librtti_b200.so")
-SOURCES = ["common.cu", "elementwise.cu", "attn_fwd.cu", "gemm_geglu.cu", "attn_probs_mean.cu", "gather_blend.cu", "vae_kernels.cu", "stripe_exchange.cu", "peer_push.cu"]
+SOURCES = ["common.cu", "elementwise.cu", "attn_fwd.cu", "gemm_geglu.cu", "attn_probs_mean.cu", "gather_blend.cu", "vae_kernels.cu", "stripe_exchange.cu", "peer_push.cu", "kmeans.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Wno-deprecated-gpu-targets",

@@ -507,3 +507,31 @@ def add_bias_f16(a, b, bias=None, out=None):
     _lib.check(lib.rtti_add_bias_f16(_ptr(a), _ptr(b), _ptr(bias), _ptr(out), a.numel() // C, C, _stream()), "rtti_add_bias_f16")
     _count(1)
     return out
+
+
+def kmeans_fit(x, draws, max_iter=300, tol=1e-4):
+    """k-means restarts of x [n, k] fp32 (rtti_kmeans_fit): draws [n_init, 1 + (k-1)*trials] fp64 from
+    attention_utils.kmeans_draws. Returns (labels [n_init, n] int32, inertia [n_init] fp64, n_iter [n_init] int32,
+    flags [n_init] int32); a non-zero flag marks a restart whose empty-cluster relocation scikit-learn leaves to an
+    unspecified order."""
+    _req(x, torch.float32, "x")
+    _req(draws, torch.float64, "draws")
+    x, draws = x.contiguous(), draws.contiguous()
+    n, k = x.shape
+    n_init = draws.shape[0]
+    if draws.dim() != 2 or draws.shape[1] != 1 + (k - 1) * (2 + int(math.log(k))):
+        raise _lib.RttiError(f"draws must be [n_init, 1 + (k-1)*trials] for k={k}, got {tuple(draws.shape)}")
+    labels = torch.empty(n_init, n, dtype=torch.int32, device=x.device)
+    inertia = torch.empty(n_init, dtype=torch.float64, device=x.device)
+    n_iter = torch.empty(n_init, dtype=torch.int32, device=x.device)
+    flags = torch.empty(n_init, dtype=torch.int32, device=x.device)
+    lib = _lib.load()
+    _lib.check(lib.rtti_kmeans_fit(_ptr(x), _ptr(draws), n, k, n_init, int(max_iter), float(tol), _ptr(labels),
+                                   _ptr(inertia), _ptr(n_iter), _ptr(flags), _stream()), "rtti_kmeans_fit")
+    _count(1)
+    return labels, inertia, n_iter, flags
+
+
+def kmeans_supported(n, k):
+    """Whether rtti_kmeans_fit accepts an [n, k] embedding (host-only query, no GPU needed)."""
+    return _lib.load().rtti_kmeans_supported(int(n), int(k)) == _lib.RTTI_OK
