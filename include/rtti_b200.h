@@ -49,6 +49,9 @@ int rtti_arch_ok(void);
  *   pbar_accum [n_slots, n_q, n_k] fp32 (device), cap_slot (host, [batch], -1 = skip):
  *       pbar_accum[cap_slot[b]] += mean over heads of P[b]  — the token-map capture of
  *       region_diffusion_sdxl.py:965-992 without the D2H copy. Deterministic. Needs n_k <= 80.
+ *       Each slot is -1..127 and no two entries may name the same slot >= 0 (their updates would race);
+ *       RTTI_ERR_ARG otherwise, as for a qk_src[b] outside [0, batch). Both host arrays are checked
+ *       before the device is queried, so the rule holds without a GPU.
  *   lse [batch, heads, n_q] fp32 or NULL: log2-domain log-sum-exp of the scaled scores
  *       (consumed by rtti_attn_probs_mean_accum).
  */

@@ -353,6 +353,21 @@ extern "C" int rtti_attn_fwd(const void* q, const void* k, const void* v, void* 
   const bool want_cap = (pbar_accum != nullptr && cap_slot != nullptr);
   if ((want_fs || want_cap) && n_k > 80) return RTTI_ERR_SHAPE;  // normalised-P features need one key tile
   if (want_fs && (!word_pos || !font_size)) return RTTI_ERR_ARG;
+  if (qk_src)
+    for (int i = 0; i < batch; ++i)
+      if (qk_src[i] < 0 || qk_src[i] >= batch) return RTTI_ERR_ARG;
+  if (want_cap) {
+    // pbar_accum[slot] += is a plain read-modify-write by the CTAs of one entry: two entries naming the same slot
+    // would race and lose updates, so every captured entry needs a slot of its own (and one that fits the int8 copy)
+    unsigned long long used[2] = {0ull, 0ull};
+    for (int i = 0; i < batch; ++i) {
+      const int s = cap_slot[i];
+      if (s < -1 || s > 127) return RTTI_ERR_ARG;
+      if (s < 0) continue;
+      if ((used[s >> 6] >> (s & 63)) & 1ull) return RTTI_ERR_ARG;
+      used[s >> 6] |= 1ull << (s & 63);
+    }
+  }
   int rc = rtti_arch_ok();
   if (rc != RTTI_OK) return rc;
   static const int n_sm = [] {
@@ -381,10 +396,7 @@ extern "C" int rtti_attn_fwd(const void* q, const void* k, const void* v, void* 
   p.inv_heads = 1.f / (float)heads;
   for (int i = 0; i < 64; ++i) { p.qk_src[i] = (int8_t)i; p.cap_slot[i] = -1; }
   if (qk_src)
-    for (int i = 0; i < batch; ++i) {
-      if (qk_src[i] < 0 || qk_src[i] >= batch) return RTTI_ERR_ARG;
-      p.qk_src[i] = (int8_t)qk_src[i];
-    }
+    for (int i = 0; i < batch; ++i) p.qk_src[i] = (int8_t)qk_src[i];   // range checked above
   if (want_cap)
     for (int i = 0; i < batch; ++i) p.cap_slot[i] = (int8_t)cap_slot[i];
   p.fs_mask = want_fs ? fs_batch_mask : 0ull;

@@ -220,16 +220,15 @@ CASES = {
     "d160_cross": lambda: attn_case(2, 8, 160, 64, 77, fs=True),
     "d32": lambda: attn_case(2, 2, 32, 64, 64),
     "d8": lambda: attn_case(2, 4, 8, 64, 77),
-    # self-attention over <= 80 tokens (an 8x8 mid block) takes the one-key-tile path: with a requested log-sum-exp /
-    # token-map capture recompute, and with injected probabilities (regression: round 2 routed both to the streaming
-    # cross kernel, which has neither)
+    # self-attention over <= 80 tokens (an 8x8 mid block) takes the single-key-tile path of attn_fwd.cu: with a
+    # requested log-sum-exp / token-map capture recompute, and with injected probabilities
     "self_64tok_lse_pm": lambda: attn_case(2, 8, 32, 64, 64, want_lse=True),
     "self_64tok_inject": lambda: attn_case(4, 8, 32, 64, 64, qk_src=[0, 1, 1, 1]),
     # Q / K handed over from another tensor (pass D's slab in a RemoteQK receive buffer): q, k batch 1, v batch 3
     "self_remote_qk": lambda: remote_qk_case(),
     "cross_xl64": lambda: attn_case(8, 10, 64, 4096, 77),
     "self_xl32": lambda: attn_case(8, 20, 64, 1024, 1024, fused_qkv=True),
-    # grouped PV (attn_self.cu): entries sharing a score source are served by one softmax
+    # injection (qk_src): entries that share a score source, each recomputing its source's softmax for its own V
     "self_group5": lambda: attn_case(8, 2, 64, 512, 512, qk_src=[0, 1, 2, 3, 3, 3, 3, 3], fused_qkv=True),
     "self_group3": lambda: attn_case(6, 2, 64, 320, 320, qk_src=[0, 1, 2, 3, 3, 3]),
     "self_group2_lse": lambda: attn_case(3, 4, 64, 200, 200, qk_src=[0, 1, 1], want_lse=True),
@@ -239,14 +238,12 @@ CASES = {
     "self_group5_xl32": lambda: attn_case(8, 20, 64, 1024, 1024, qk_src=[0, 1, 2, 3, 3, 3, 3, 3], fused_qkv=True),
     "self_rescale": lambda: rescale_case(),
     "sanitizer_small": lambda: case_sanitizer_small(),
-    # grouping disabled (RTTI_ATTN_MAX_GROUP=1): every entry evaluates its own softmax from its source's Q, K
-    "g1:self_group5": lambda: attn_case(8, 2, 64, 512, 512, qk_src=[0, 1, 2, 3, 3, 3, 3, 3], fused_qkv=True),
 }
 
 
 def remote_qk_case():
     """ops.attention with q / k of batch 1 (another pass's Q|K slab, strided like a [1, T, 2C] receive buffer) and v of
-    batch 3: every entry applies softmax(q k^T) of entry 0 to its own values — plain (1 entry) and grouped (3 entries)."""
+    batch 3: every entry applies softmax(q k^T) of entry 0 to its own values — one entry and three entries."""
     import torch
     from rtti_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(5)
@@ -264,7 +261,8 @@ def remote_qk_case():
 
 
 def rescale_case():
-    """Row maxima that grow by far more than 2^8 from key tile to key tile: exercises the lazy O rescale (plain and grouped)."""
+    """Row maxima that grow by far more than 2^8 from key tile to key tile: exercises the online O rescale (with and
+    without injection)."""
     import torch
     from rtti_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(3)
@@ -284,14 +282,14 @@ def rescale_case():
 
 
 def case_sanitizer_small():
-    """Small shapes of every kernel family for compute-sanitizer (memcheck / racecheck run 10-100x slower)."""
+    """Small shapes of every kernel family in one process."""
     import torch
     from rtti_b200 import ops
     ok = True
-    ok &= attn_case(2, 2, 64, 256, 256)                                  # plain self-attention (3 CTAs/SM kernel)
-    ok &= attn_case(4, 2, 64, 192, 192, qk_src=[0, 1, 1, 1])             # grouped self-attention (2 threads per row)
+    ok &= attn_case(2, 2, 64, 256, 256)                                  # self-attention, 64-key tiles
+    ok &= attn_case(4, 2, 64, 192, 192, qk_src=[0, 1, 1, 1])             # self-attention with injection
     ok &= attn_case(2, 2, 64, 128, 77, fs=True, cap=True)                # cross-attention, font sizes + capture
-    ok &= attn_case(1, 2, 80, 128, 128, want_lse=True)                   # head_dim 80 (128-key-tile kernel) + probs mean
+    ok &= attn_case(1, 2, 80, 128, 128, want_lse=True)                   # head_dim 80 (two d-chunks) + probs mean
     x = (torch.randn(2, 256, 64, device="cuda") * 2).half(); ga = torch.randn(64, device="cuda").half(); be = torch.randn(64, device="cuda").half()
     ops.groupnorm_silu(x, ga, be, 8, 1e-5, True)
     ops.layernorm(x, ga, be, 1e-5)
@@ -314,14 +312,6 @@ def case_sanitizer_small():
     return ok
 
 
-def case_env(name):
-    """Environment of the subprocess that runs case `name` ("g1:" prefix = grouping disabled, every entry its own softmax)."""
-    env = dict(os.environ)
-    if name.startswith("g1:"):
-        env["RTTI_ATTN_MAX_GROUP"] = "1"
-    return env
-
-
 if __name__ == "__main__":
     if len(sys.argv) > 2 and sys.argv[1] == "--many":   # several cases in ONE process (bring-up; wrap in `timeout`)
         bad = []
@@ -332,14 +322,12 @@ if __name__ == "__main__":
         print("MANY", "ALL PASS" if not bad else f"FAILED {bad}", flush=True)
         sys.exit(1 if bad else 0)
     if len(sys.argv) > 1:
-        os.environ.update(case_env(sys.argv[1]))   # the library reads its switches at load time (first op call)
         ok = CASES[sys.argv[1]]()
         sys.exit(0 if ok else 1)
     summary = []
     for name in CASES:
         try:
-            env = case_env(name)
-            r = subprocess.run([sys.executable, os.path.abspath(__file__), name], timeout=120, capture_output=True, text=True, env=env)
+            r = subprocess.run([sys.executable, os.path.abspath(__file__), name], timeout=120, capture_output=True, text=True)
             out = (r.stdout + r.stderr).strip()
             status = "ok" if r.returncode == 0 else f"rc={r.returncode}"
         except subprocess.TimeoutExpired as e:

@@ -7,37 +7,16 @@ Tolerance rule, used throughout: for each op compute
   * the kernel / engine result,
 and require err_kernel <= K * err_torch32 + floor with err = max|x - ref64| and floor a few fp32 ulps of the output
 range (half an fp16 ulp for fp16 outputs). That is: no worse than the implementation it replaces, at the same
-precision. A fixed absolute tolerance would let a kernel that is several times less accurate pass.
+precision. A fixed absolute tolerance would let a kernel that is several times less accurate pass. The rule lives in
+tests/fp64_rule.py, shared with tests/test_unet_kernels_fp64.py.
 Every case prints both errors ("[fp64] ..." lines, visible with -s)."""
 import ctypes
-import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
-EPS32 = torch.finfo(torch.float32).eps
-
-
-def _maxerr(got, ref):
-    """max |got - ref| in float64, in slices (the SDXL activations are up to 256M elements)."""
-    a, b = got.reshape(-1), ref.reshape(-1)
-    step = 1 << 25
-    return max(float((a[i:i + step].double() - b[i:i + step]).abs().max()) for i in range(0, a.numel(), step))
-
-
-def _absmax(t):
-    return float(t.abs().max())
-
-
-def _no_worse(what, got, torch32, ref, k=4.0, floor_ulps=4.0, floor=None):
-    e_k, e_t = _maxerr(got, ref), _maxerr(torch32, ref)
-    if floor is None:
-        floor = floor_ulps * EPS32 * _absmax(ref)
-    print(f"[fp64] {what}: kernel {e_k:.3e}  torch {e_t:.3e}  (ref absmax {_absmax(ref):.3g})")
-    assert math.isfinite(e_k) and e_k <= k * e_t + floor, (
-        f"{what}: kernel err {e_k:.3e} > {k:g} x torch fp32 err {e_t:.3e} + floor {floor:.3e}")
-    return e_k, e_t
+from tests.fp64_rule import EPS32, absmax as _absmax, half_ulp16, no_worse as _no_worse
 
 
 def _gen(seed):
@@ -168,10 +147,16 @@ def test_fp16_groupnorm_abi_rejects_more_than_1024_threads_without_launching():
 @pytest.mark.parametrize("offset", OFFSETS)
 def test_fp16_groupnorm_statistics_hold_for_offset_inputs(B, HW, C, temb, offset):
     """rtti_groupnorm_silu_fwd (UNet, fp16 in/out, fp32 statistics) on x = randn + offset, the offset in x or in the
-    temb chan_bias, at two UNet shapes and at c = 8192 (1024 threads per CTA, the largest the entry point accepts). Reference: float64 on the same fp16 inputs; PyTorch: fp32 GroupNorm + SiLU rounded to fp16.
-    Floor: the fp16 output rounding, half an fp16 ulp of max|y|."""
+    temb chan_bias, at two UNet shapes and at c = 8192 (1024 threads per CTA, the largest the entry point accepts)."""
+    check_fp16_groupnorm(B, HW, C, temb, offset, seed=int(offset) + C + temb)
+
+
+def check_fp16_groupnorm(B, HW, C, temb, offset, seed, k=4.0, mean=False):
+    """ops.groupnorm_silu (G = 32, SiLU) on x = randn + offset, the offset in x or in the temb chan_bias. Reference:
+    float64 on the same fp16 inputs; PyTorch: fp32 GroupNorm + SiLU rounded to fp16. Floor: the fp16 output rounding,
+    half an fp16 ulp of max|y|."""
     from rtti_b200 import ops
-    g = _gen(int(offset) + C + temb)
+    g = _gen(seed)
     G, eps = 32, 1e-5
     x = torch.randn(B, HW, C, device="cuda", generator=g)
     cb = None
@@ -190,8 +175,8 @@ def test_fp16_groupnorm_statistics_hold_for_offset_inputs(B, HW, C, temb, offset
     y64 = ref(torch.float64)
     y32 = ref(torch.float32).half()
     y = ops.groupnorm_silu(x, ga, be, G, eps, True, chan_bias=cb)
-    half_ulp = 2.0 ** (math.floor(math.log2(_absmax(y64))) - 11)
-    _no_worse(f"fp16 groupnorm B{B} HW{HW} C{C} temb={temb} offset={offset:g}", y, y32, y64, floor=half_ulp)
+    _no_worse(f"fp16 groupnorm B{B} HW{HW} C{C} temb={temb} offset={offset:g}", y, y32, y64, floor=half_ulp16(y64),
+              k=k, mean=mean)
 
 
 # ------------------------------------------------------------------------------------------------ c. striped, world 1

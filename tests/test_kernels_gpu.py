@@ -16,6 +16,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.mark.parametrize("case", list(gpu_diag.CASES))
 def test_kernel_case(case):
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "gpu_diag.py"), case], capture_output=True, text=True,
-                       timeout=300, env=gpu_diag.case_env(case))
+                       timeout=300)
     assert r.returncode == 0, (r.stdout + r.stderr)[-3000:]
     assert "FAIL" not in r.stdout
