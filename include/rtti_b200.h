@@ -127,6 +127,19 @@ int rtti_region_blend_cfg(const void* eps_uncond, const void* const* eps_region,
                           int n_regions, long long n, float guidance, void* eps_out, const void* latents,
                           void* latents_out, float dt_sigma, void* stream);
 
+/* rtti_region_blend_cfg with the CFG rescale of diffusers' rescale_noise_cfg (models/region_diffusion_sdxl.py:42-53,
+ * applied at :903-905; the rich-text loop's call left as a TODO at :827-830):
+ *   eps = eps_cfg * (1 - guidance_rescale + guidance_rescale * std(eps_t) / std(eps_cfg))
+ * with eps_t the blended text prediction and eps_cfg = eps_u + guidance * (eps_t - eps_u), the unbiased standard
+ * deviations taken over all n elements in fp32 from the fp32 values; eps is rounded to fp16 before it is stored and
+ * before the Euler update consumes it. std(eps_cfg) = 0 gives a non-finite result, as the formula does.
+ * One launch of one 8-CTA thread-block cluster (the statistics are merged in a fixed order through distributed shared
+ * memory: deterministic, no workspace, no atomics). n a multiple of 8 and <= 262144 (RTTI_ERR_SHAPE otherwise),
+ * n_regions <= 16; all pointers 16-byte aligned. */
+int rtti_region_blend_cfg_rescale(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                  int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                  void* latents_out, float dt_sigma, float guidance_rescale, void* stream);
+
 /* Colour-guidance loss forward + analytic backward w.r.t. the VAE decoder output.
  * Replaces models/region_diffusion_sdxl.py:857-865 (clamp, masked mean RGB, MSE*100, autograd of those).
  *   decoded [3, hw] fp32 (VAE output before /2+0.5), masks [n_colors, hw] fp32 (channel 0 of
@@ -201,6 +214,16 @@ int rtti_gather_blend_step(const void* const* peer_slots, void* const* peer_flag
                            float guidance, void* eps_out, const void* latents, void* latents_out,
                            const void* latents_ref, void* latents_ref_out, float dt_sigma, unsigned int step_id,
                            void* stream);
+/* rtti_gather_blend_step with the CFG rescale of rtti_region_blend_cfg_rescale, same protocol and slot layout. The
+ * reference-latent pair, when latents_ref is given, is rescaled on its own statistics (eps_t = eps_D,
+ * eps_cfg = eps_C + guidance * (eps_D - eps_C)). For the same noise predictions the outputs equal those of
+ * rtti_region_blend_cfg_rescale (the C/D pair: called with one region and a mask of ones) bit for bit, whatever the
+ * world size. n a multiple of 8 and <= 262144 (RTTI_ERR_SHAPE otherwise); masks and outputs 16-byte aligned. */
+int rtti_gather_blend_step_rescale(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                   const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                                   float guidance, void* eps_out, const void* latents, void* latents_out,
+                                   const void* latents_ref, void* latents_ref_out, float dt_sigma,
+                                   unsigned int step_id, float guidance_rescale, void* stream);
 
 /* Stripe-parallel colour guidance (multi-GPU; new relative to the single-GPU reference, which back-propagates
  * through the batch-1 VAE decoder on one device: models/region_diffusion_sdxl.py:849-867). Every activation of

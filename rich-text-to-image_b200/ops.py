@@ -220,9 +220,11 @@ def geglu(proj, out=None):
     return out
 
 
-def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0):
+def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0):
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
-    eps_regions: list of fp16 tensors (region passes in mask order, base-prompt pass last); masks fp32 [N, n]."""
+    eps_regions: list of fp16 tensors (region passes in mask order, base-prompt pass last); masks fp32 [N, n].
+    guidance_rescale = phi > 0 scales eps by 1 - phi + phi std(eps_t) / std(eps) before it is stored and stepped
+    (rtti_region_blend_cfg_rescale); phi == 0 runs rtti_region_blend_cfg."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -233,9 +235,15 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    rc = lib.rtti_region_blend_cfg(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
-                                   _ptr(latents), _ptr(lat_out), float(dt_sigma), _stream())
-    _lib.check(rc, "rtti_region_blend_cfg")
+    if guidance_rescale == 0.0:
+        rc = lib.rtti_region_blend_cfg(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
+                                       _ptr(latents), _ptr(lat_out), float(dt_sigma), _stream())
+        _lib.check(rc, "rtti_region_blend_cfg")
+    else:
+        rc = lib.rtti_region_blend_cfg_rescale(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
+                                               _ptr(latents), _ptr(lat_out), float(dt_sigma), float(guidance_rescale),
+                                               _stream())
+        _lib.check(rc, "rtti_region_blend_cfg_rescale")
     _count(1)
     return (eps_out, lat_out) if latents is not None else eps_out
 
@@ -304,8 +312,9 @@ def predict_x0(x_t, eps, alpha):
 
 
 def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_regions, masks, guidance, latents, latents_ref,
-                      dt_sigma, step_id):
-    """Fused all-gather + blend + CFG + Euler over NVLink peer memory (rtti_gather_blend_step).
+                      dt_sigma, step_id, guidance_rescale=0.0):
+    """Fused all-gather + blend + CFG + Euler over NVLink peer memory (rtti_gather_blend_step; with
+    guidance_rescale > 0 rtti_gather_blend_step_rescale, which also rescales the reference-latent pair).
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
@@ -316,10 +325,17 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    rc = lib.rtti_gather_blend_step(slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions,
-                                    _ptr(masks), n, float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out),
-                                    _ptr(latents_ref), _ptr(ref_out), float(dt_sigma), int(step_id), _stream())
-    _lib.check(rc, "rtti_gather_blend_step")
+    if guidance_rescale == 0.0:
+        rc = lib.rtti_gather_blend_step(slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions,
+                                        _ptr(masks), n, float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out),
+                                        _ptr(latents_ref), _ptr(ref_out), float(dt_sigma), int(step_id), _stream())
+        _lib.check(rc, "rtti_gather_blend_step")
+    else:
+        rc = lib.rtti_gather_blend_step_rescale(slots, flags, world, rank, _int_array(slot_owner), len(slot_owner),
+                                                n_regions, _ptr(masks), n, float(guidance), _ptr(eps), _ptr(latents),
+                                                _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out), float(dt_sigma),
+                                                int(step_id), float(guidance_rescale), _stream())
+        _lib.check(rc, "rtti_gather_blend_step_rescale")
     _count(1)
     return eps, lat_out, ref_out
 

@@ -7,7 +7,8 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
   * the 2 + 2*inject + (N-1) UNet passes of a step (uncond, base+font-size, reference uncond, reference
     base, N-1 regions; :787-821) run as ONE batched UNet call — they share the timestep and, up to the
     reference latent, the input; the hook choreography becomes a RegionControl;
-  * region blend + CFG + Euler update is one kernel (rtti_region_blend_cfg); colour-guidance loss fwd/bwd,
+  * region blend + CFG (+ guidance rescale) + Euler update is one kernel (rtti_region_blend_cfg, or
+    rtti_region_blend_cfg_rescale with guidance_rescale > 0); colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
     per-pass noise predictions are all-gathered before the (replicated, deterministic) blend.
@@ -23,6 +24,11 @@ from .attention_utils import CrossAttentionLayers_XL
 from .schedulers import EulerDiscreteScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
+
+
+def _rescale_phi(guidance_scale, guidance_rescale):
+    """The guidance rescale in effect: the reference applies it only with classifier-free guidance on (:903)."""
+    return float(guidance_rescale) if guidance_scale > 1.0 and guidance_rescale > 0.0 else 0.0
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -184,13 +190,13 @@ class RegionDiffusionXL:
                inject_selfattn: float = 0.0, inject_background: float = 0.0, text_format_dict: Optional[dict] = None,
                run_rich_text: bool = False):
         """Signature of models/region_diffusion_sdxl.py:556-587. `prompt` is the list of region prompts with the
-        base prompt last (sample.py:107); embeddings may be passed instead of text."""
+        base prompt last (sample.py:107); embeddings may be passed instead of text. `guidance_rescale` (applied when
+        guidance_scale > 1) rescales the CFG prediction as diffusers' rescale_noise_cfg in both passes; the reference
+        implements it for the plain pass only (:903-905) and raises NotImplementedError in the rich-text pass (:827-830)."""
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)
         target_size = target_size or (height, width)
-        if guidance_rescale > 0.0 and run_rich_text:
-            raise NotImplementedError  # as the reference, :826-829
         if prompt_embeds is None:
             prompt_embeds, negative_prompt_embeds, pooled_prompt_embeds, negative_pooled_prompt_embeds = \
                 self.encode_prompt(prompt, negative_prompt)
@@ -207,9 +213,10 @@ class RegionDiffusionXL:
         if run_rich_text:
             latents = self._rich_text_loop(ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
                                            inject_selfattn, inject_background, text_format_dict or {}, callback,
-                                           callback_steps)
+                                           callback_steps, guidance_rescale)
         else:
-            latents = self._plain_loop(ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps)
+            latents = self._plain_loop(ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps,
+                                       guidance_rescale)
 
         if output_type == "latent":
             return StableDiffusionXLPipelineOutput(images=latents)
@@ -223,8 +230,11 @@ class RegionDiffusionXL:
         from PIL import Image
         return StableDiffusionXLPipelineOutput(images=[Image.fromarray(a) for a in arr])
 
-    def _plain_loop(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps):
-        """:879-914 — CFG batch [uncond, cond]; with capture armed the attention kernels accumulate the maps."""
+    def _plain_loop(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps,
+                    guidance_rescale=0.0):
+        """:879-914 — CFG batch [uncond, cond]; with capture armed the attention kernels accumulate the maps.
+        guidance_rescale rescales the CFG prediction inside the blend kernel (:903-905)."""
+        phi = _rescale_phi(guidance_scale, guidance_rescale)
         ctx2 = torch.cat([ctx[:1], ctx[-1:]])
         pooled2 = torch.cat([pooled[:1], pooled[-1:]])
         kv = CrossKVCache()
@@ -238,7 +248,8 @@ class RegionDiffusionXL:
             if ones is None:
                 ones = torch.ones(1, n, dtype=torch.float32, device=eps.device)
             _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                              latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t))
+                                              latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
+                                              guidance_rescale=phi)
             if callback is not None and i % callback_steps == 0:
                 callback(i, t, latents)
         return latents
@@ -255,8 +266,10 @@ class RegionDiffusionXL:
         return passes
 
     def prepare_rich_text(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
-                          inject_selfattn, inject_background, tfd):
-        """Everything of :772-778 that is constant over the steps, as a state object for rich_text_step()."""
+                          inject_selfattn, inject_background, tfd, guidance_rescale=0.0):
+        """Everything of :772-778 that is constant over the steps, as a state object for rich_text_step().
+        guidance_rescale: the CFG rescale the reference leaves as a TODO (:827-830), applied to the blended prediction
+        (eps_text = the masked sum of the text passes) and, when it is stepped, to the reference-latent pair C/D."""
         dev = self.device
         N = len(self.masks)
         assert ctx.shape[0] == N + 1, "prompts must be [region_1..region_{N-1}, base] matching self.masks"
@@ -267,6 +280,7 @@ class RegionDiffusionXL:
         st.latents_ref = latents.clone() if inject else None
         st.timesteps, st.n_t = timesteps, len(timesteps)
         st.guidance_scale, st.use_guidance = guidance_scale, use_guidance
+        st.guidance_rescale = _rescale_phi(guidance_scale, guidance_rescale)
         st.inject, st.inject_selfattn, st.inject_background = inject, inject_selfattn, inject_background
         st.tfd = tfd
         st.N = N
@@ -420,7 +434,8 @@ class RegionDiffusionXL:
             sid = ex.publish(eps_local, local, owner)
             st.noise_pred, st.latents, ref_out = ops.gather_blend_step(
                 ex.slot_ptrs, ex.flag_ptrs, ex.rank, ex.slot_owner(owner), N, st.masks, st.guidance_scale,
-                st.latents.contiguous(), st.latents_ref.contiguous() if step_ref else None, dt, sid)
+                st.latents.contiguous(), st.latents_ref.contiguous() if step_ref else None, dt, sid,
+                guidance_rescale=st.guidance_rescale)
             if step_ref:
                 st.latents_ref = ref_out
         else:
@@ -428,10 +443,12 @@ class RegionDiffusionXL:
             one = lambda name: eps[kind[name]:kind[name] + 1].contiguous()
             regions = [one(f"E{j}") for j in range(N - 1)] + [one("B")]
             st.noise_pred, st.latents = ops.region_blend_cfg(one("A"), regions, st.masks, st.guidance_scale,
-                                                              latents=st.latents.contiguous(), dt_sigma=dt)   # :810-825, :845
+                                                              latents=st.latents.contiguous(), dt_sigma=dt,
+                                                              guidance_rescale=st.guidance_rescale)   # :810-830, :845
             if step_ref:
                 _, st.latents_ref = ops.region_blend_cfg(one("C"), [one("D")], st.ones, st.guidance_scale,
-                                                         latents=st.latents_ref.contiguous(), dt_sigma=dt)
+                                                         latents=st.latents_ref.contiguous(), dt_sigma=dt,
+                                                         guidance_rescale=st.guidance_rescale)
         if pe is not None:
             ev[2].record()
         if st.use_guidance and float(t) < st.tfd["guidance_start_step"]:                                  # :849
@@ -446,10 +463,10 @@ class RegionDiffusionXL:
         return st.latents
 
     def _rich_text_loop(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
-                        inject_selfattn, inject_background, tfd, callback, callback_steps):
+                        inject_selfattn, inject_background, tfd, callback, callback_steps, guidance_rescale=0.0):
         """:772-878."""
         st = self.prepare_rich_text(ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
-                                    inject_selfattn, inject_background, tfd)
+                                    inject_selfattn, inject_background, tfd, guidance_rescale)
         for i, t in enumerate(timesteps):
             self.rich_text_step(st, i)
             if callback is not None and i % callback_steps == 0:
