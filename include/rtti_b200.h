@@ -140,6 +140,23 @@ int rtti_region_blend_cfg_rescale(const void* eps_uncond, const void* const* eps
                                   int n_regions, long long n, float guidance, void* eps_out, const void* latents,
                                   void* latents_out, float dt_sigma, float guidance_rescale, void* stream);
 
+/* Multistep forms ("_ms") of the blend entry points, for DDIM and DPM-Solver++(2M) (rich-text-to-image_b200/schedulers.py,
+ * StepCoeffs). The blend, CFG and rescale arithmetic is that of the Euler form; the update of the latents is
+ *   D  = hx * x + he * eps                (fp32, written to d_out[n])
+ *   x' = cx * x + cd * D + cp * D_prev    (D_prev = d_prev[n], read only when cp != 0; x' rounded to fp16)
+ * with x the fp16 latents and eps the fp16-rounded noise prediction written to eps_out. latents, latents_out and d_out
+ * are required; d_prev may be null only when cp == 0, and it may alias d_out (every element is read before it is
+ * written, by the same thread). d_prev / d_out 16-byte aligned. The other checks are those of the Euler form; on any
+ * error nothing is launched. */
+int rtti_region_blend_cfg_ms(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions,
+                             long long n, float guidance, void* eps_out, const void* latents, void* latents_out,
+                             float hx, float he, float cx, float cd, float cp, const float* d_prev, float* d_out,
+                             void* stream);
+int rtti_region_blend_cfg_rescale_ms(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                     int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                     void* latents_out, float hx, float he, float cx, float cd, float cp,
+                                     const float* d_prev, float* d_out, float guidance_rescale, void* stream);
+
 /* Colour-guidance loss forward + analytic backward w.r.t. the VAE decoder output.
  * Replaces models/region_diffusion_sdxl.py:857-865 (clamp, masked mean RGB, MSE*100, autograd of those).
  *   decoded [3, hw] fp32 (VAE output before /2+0.5), masks [n_colors, hw] fp32 (channel 0 of
@@ -224,6 +241,24 @@ int rtti_gather_blend_step_rescale(const void* const* peer_slots, void* const* p
                                    float guidance, void* eps_out, const void* latents, void* latents_out,
                                    const void* latents_ref, void* latents_ref_out, float dt_sigma,
                                    unsigned int step_id, float guidance_rescale, void* stream);
+
+/* Multistep forms of the two gather entry points (see rtti_region_blend_cfg_ms). The reference-latent trajectory, when
+ * latents_ref is given, is stepped with the same coefficients on its own history (d_prev_ref -> d_out_ref, required
+ * then), so each trajectory keeps its own D. For the same noise predictions the outputs equal those of the single-GPU
+ * forms (the C/D pair: one region and a mask of ones) bit for bit, whatever the world size. */
+int rtti_gather_blend_step_ms(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                              const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                              float guidance, void* eps_out, const void* latents, void* latents_out,
+                              const void* latents_ref, void* latents_ref_out, float hx, float he, float cx, float cd,
+                              float cp, const float* d_prev, float* d_out, const float* d_prev_ref, float* d_out_ref,
+                              unsigned int step_id, void* stream);
+int rtti_gather_blend_step_rescale_ms(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                      const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                      long long n, float guidance, void* eps_out, const void* latents,
+                                      void* latents_out, const void* latents_ref, void* latents_ref_out, float hx,
+                                      float he, float cx, float cd, float cp, const float* d_prev, float* d_out,
+                                      const float* d_prev_ref, float* d_out_ref, unsigned int step_id,
+                                      float guidance_rescale, void* stream);
 
 /* Stripe-parallel colour guidance (multi-GPU; new relative to the single-GPU reference, which back-propagates
  * through the batch-1 VAE decoder on one device: models/region_diffusion_sdxl.py:849-867). Every activation of

@@ -20,6 +20,8 @@
 #include <cooperative_groups.h>
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "rtti_internal.h"
 
 namespace rtti {
@@ -51,6 +53,23 @@ struct RescaleParams {
   int world, rank;
   unsigned int step_id;
 };
+
+// the multistep form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory
+struct RescaleMsParams : RescaleParams {
+  MsStep ms, ms_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep update of the main (REF false) / reference
+// (REF true) trajectory
+template <bool REF>
+__device__ __forceinline__ void rs_step(const RescaleParams& p, long long, const float* e16, float* x) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
+}
+template <bool REF>
+__device__ __forceinline__ void rs_step(const RescaleMsParams& p, long long v, const float* e16, float* x) {
+  ms_step8(REF ? p.ms_ref : p.ms, v, e16, x);
+}
 
 // (count, mean, m2) of eps_text and of eps_cfg over the same elements
 struct PairStats { int n; float mt, qt, mc, qc; };
@@ -87,8 +106,8 @@ __device__ __forceinline__ void load8(const __half* p, float* f) {
 
 // eps_text = sum_r m_r eps_r and eps_cfg = u + g (eps_text - u), u = eps_uncond * sum_r m_r, for vector v: the
 // arithmetic of region_blend_kernel. ONES: every mask is 1 (the C/D pair, as the single-GPU path blends it).
-template <bool PEER, bool ONES>
-__device__ __forceinline__ void blend_vec(const RescaleParams& p, int s0, int n_reg, long long v, float* et, float* ec) {
+template <bool PEER, bool ONES, class P>
+__device__ __forceinline__ void blend_vec(const P& p, int s0, int n_reg, long long v, float* et, float* ec) {
   float msum[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) { msum[i] = 0.f; et[i] = 0.f; }
@@ -130,9 +149,10 @@ struct RescaleSmem {
 };
 
 // One reduction + apply over the whole image: slots s0 (uncond) and s0+1..s0+n_reg, outputs eps_out (may be null) and
-// lat_out = lat + dt_sigma * eps (when lat is non-null). Vector v = (k * RS_CL + cta rank) * threads + thread, k < vpt.
-template <bool PEER, bool ONES>
-__device__ void rescale_job(const RescaleParams& p, int s0, int n_reg, __half* eps_out, const __half* lat,
+// lat_out = lat stepped with eps (when lat is non-null; the reference trajectory's step when ONES). Vector
+// v = (k * RS_CL + cta rank) * threads + thread, k < vpt.
+template <bool PEER, bool ONES, class P>
+__device__ void rescale_job(const P& p, int s0, int n_reg, __half* eps_out, const __half* lat,
                             __half* lat_out, float4* cfg_s, RescaleSmem& sm) {
   cg::cluster_group cluster = cg::this_cluster();
   const int tid = threadIdx.x, T = p.threads, crank = (int)cluster.block_rank();
@@ -185,19 +205,15 @@ __device__ void rescale_job(const RescaleParams& p, int s0, int n_reg, __half* e
         float x[8], e16[8];
         unpack8(*reinterpret_cast<const uint4*>(lat + v * 8), x);
         unpack8(oh, e16);  // the scheduler consumes the fp16-rounded noise prediction
-#pragma unroll
-        for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
+        rs_step<ONES>(p, v, e16, x);
         *reinterpret_cast<uint4*>(lat_out + v * 8) = pack8(x);
       }
     }
   }
 }
 
-template <bool PEER>
-__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
-    blend_rescale_kernel(const __grid_constant__ RescaleParams p) {
-  extern __shared__ float4 cfg_s[];
-  __shared__ RescaleSmem sm;
+template <bool PEER, class P>
+__device__ __forceinline__ void blend_rescale_body(const P& p, float4* cfg_s, RescaleSmem& sm) {
   if constexpr (PEER) {
     // gather_blend.cu's protocol: publish this rank's step, wait (acquire, ~4 s timeout) for every peer's
     if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -225,6 +241,22 @@ __global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
     rescale_job<PEER, true>(p, p.n_regions + 1, 1, nullptr, p.latents_ref, p.latents_ref_out, cfg_s, sm);
 }
 
+template <bool PEER>
+__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
+    blend_rescale_kernel(const __grid_constant__ RescaleParams p) {
+  extern __shared__ float4 cfg_s[];
+  __shared__ RescaleSmem sm;
+  blend_rescale_body<PEER>(p, cfg_s, sm);
+}
+
+template <bool PEER>
+__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
+    blend_rescale_ms_kernel(const __grid_constant__ RescaleMsParams p) {
+  extern __shared__ float4 cfg_s[];
+  __shared__ RescaleSmem sm;
+  blend_rescale_body<PEER>(p, cfg_s, sm);
+}
+
 // threads per CTA and vectors per thread: a function of n only
 void rescale_plan(long long n, int& threads, int& vpt) {
   const long long nv = n / 8, per_cta = (nv + RS_CL - 1) / RS_CL;
@@ -237,30 +269,28 @@ void rescale_plan(long long n, int& threads, int& vpt) {
   }
 }
 
-template <bool PEER>
-int launch_rescale(RescaleParams& p, void* stream) {
+template <bool PEER, class P>
+int launch_rescale(P& p, void* stream) {
+  constexpr bool MS = !std::is_same<P, RescaleParams>::value;
   static const bool configured =
-      cudaFuncSetAttribute(blend_rescale_kernel<PEER>, cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM) == cudaSuccess;
+      cudaFuncSetAttribute(MS ? (const void*)blend_rescale_ms_kernel<PEER> : (const void*)blend_rescale_kernel<PEER>,
+                           cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM) == cudaSuccess;
   if (!configured) return RTTI_ERR_CUDA;
   rescale_plan(p.n, p.threads, p.vpt);
-  blend_rescale_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
+  if constexpr (MS)
+    blend_rescale_ms_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
+  else
+    blend_rescale_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }
 
-}  // namespace
-}  // namespace rtti
-
-using namespace rtti;
-
-extern "C" int rtti_region_blend_cfg_rescale(const void* eps_uncond, const void* const* eps_region, const float* masks,
-                                             int n_regions, long long n, float guidance, void* eps_out,
-                                             const void* latents, void* latents_out, float dt_sigma,
-                                             float guidance_rescale, void* stream) {
+// argument checks of the single-GPU entry points; fills everything but the step and the rescale factor
+int rescale_args(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions, long long n,
+                 float guidance, void* eps_out, const void* latents, void* latents_out, RescaleParams& p) {
   if (!eps_uncond || !eps_region || !masks || !eps_out) return RTTI_ERR_ARG;
   if (n_regions < 1 || n_regions > RS_MAX_REGIONS || n < 8) return RTTI_ERR_ARG;
   if (n % 8 != 0 || n > RS_MAX_N) return RTTI_ERR_SHAPE;
   if ((latents == nullptr) != (latents_out == nullptr)) return RTTI_ERR_ARG;
-  RescaleParams p{};
   uintptr_t al = (uintptr_t)eps_uncond | (uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out;
   p.slot[0] = (const __half*)eps_uncond;
   for (int i = 0; i < n_regions; ++i) {
@@ -269,18 +299,16 @@ extern "C" int rtti_region_blend_cfg_rescale(const void* eps_uncond, const void*
     al |= (uintptr_t)eps_region[i];
   }
   if (al & 15) return RTTI_ERR_ALIGN;
-  p.masks = masks; p.n_regions = n_regions; p.n = n;
-  p.guidance = guidance; p.phi = guidance_rescale; p.dt_sigma = dt_sigma;
+  p.masks = masks; p.n_regions = n_regions; p.n = n; p.guidance = guidance;
   p.eps_out = (__half*)eps_out; p.latents = (const __half*)latents; p.latents_out = (__half*)latents_out;
-  return launch_rescale<false>(p, stream);
+  return RTTI_OK;
 }
 
-extern "C" int rtti_gather_blend_step_rescale(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
-                                              const int* slot_owner, int n_slots, int n_regions, const float* masks,
-                                              long long n, float guidance, void* eps_out, const void* latents,
-                                              void* latents_out, const void* latents_ref, void* latents_ref_out,
-                                              float dt_sigma, unsigned int step_id, float guidance_rescale,
-                                              void* stream) {
+// argument checks of the gather entry points; fills everything but the step and the rescale factor
+int gather_rescale_args(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                        const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                        float guidance, void* eps_out, const void* latents, void* latents_out, const void* latents_ref,
+                        void* latents_ref_out, unsigned int step_id, RescaleParams& p) {
   if (!peer_slots || !peer_flags || !slot_owner || !masks || !eps_out) return RTTI_ERR_ARG;
   if (world < 1 || world > RS_MAX_WORLD || rank < 0 || rank >= world) return RTTI_ERR_ARG;
   if (n_regions < 1 || n_slots < n_regions + 1 || n_slots > RS_MAX_SLOTS || n < 8) return RTTI_ERR_ARG;
@@ -291,7 +319,6 @@ extern "C" int rtti_gather_blend_step_rescale(const void* const* peer_slots, voi
   if (((uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out | (uintptr_t)latents_ref |
        (uintptr_t)latents_ref_out) & 15)
     return RTTI_ERR_ALIGN;
-  RescaleParams p{};
   for (int r = 0; r < world; ++r) {
     if (!peer_slots[r] || !peer_flags[r]) return RTTI_ERR_ARG;
     if ((uintptr_t)peer_slots[r] & 15) return RTTI_ERR_ALIGN;
@@ -303,9 +330,74 @@ extern "C" int rtti_gather_blend_step_rescale(const void* const* peer_slots, voi
     p.slot[s] = (const __half*)peer_slots[slot_owner[s]] + par + (size_t)s * n;
   }
   p.world = world; p.rank = rank; p.step_id = step_id;
-  p.masks = masks; p.n_regions = n_regions; p.n = n;
-  p.guidance = guidance; p.phi = guidance_rescale; p.dt_sigma = dt_sigma;
+  p.masks = masks; p.n_regions = n_regions; p.n = n; p.guidance = guidance;
   p.eps_out = (__half*)eps_out; p.latents = (const __half*)latents; p.latents_out = (__half*)latents_out;
   p.latents_ref = (const __half*)latents_ref; p.latents_ref_out = (__half*)latents_ref_out;
+  return RTTI_OK;
+}
+
+}  // namespace
+}  // namespace rtti
+
+using namespace rtti;
+
+extern "C" int rtti_region_blend_cfg_rescale(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                             int n_regions, long long n, float guidance, void* eps_out,
+                                             const void* latents, void* latents_out, float dt_sigma,
+                                             float guidance_rescale, void* stream) {
+  RescaleParams p{};
+  const int rc = rescale_args(eps_uncond, eps_region, masks, n_regions, n, guidance, eps_out, latents, latents_out, p);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale; p.dt_sigma = dt_sigma;
+  return launch_rescale<false>(p, stream);
+}
+
+extern "C" int rtti_region_blend_cfg_rescale_ms(const void* eps_uncond, const void* const* eps_region,
+                                                const float* masks, int n_regions, long long n, float guidance,
+                                                void* eps_out, const void* latents, void* latents_out, float hx,
+                                                float he, float cx, float cd, float cp, const float* d_prev,
+                                                float* d_out, float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleMsParams p{};
+  int rc = rescale_args(eps_uncond, eps_region, masks, n_regions, n, guidance, eps_out, latents, latents_out, p);
+  if (rc == RTTI_OK) rc = ms_step_args(cp, d_prev, d_out);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.ms = MsStep{hx, he, cx, cd, cp, d_prev, d_out};
+  return launch_rescale<false>(p, stream);
+}
+
+extern "C" int rtti_gather_blend_step_rescale(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                              const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                              long long n, float guidance, void* eps_out, const void* latents,
+                                              void* latents_out, const void* latents_ref, void* latents_ref_out,
+                                              float dt_sigma, unsigned int step_id, float guidance_rescale,
+                                              void* stream) {
+  RescaleParams p{};
+  const int rc = gather_rescale_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n,
+                                     guidance, eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale; p.dt_sigma = dt_sigma;
+  return launch_rescale<true>(p, stream);
+}
+
+extern "C" int rtti_gather_blend_step_rescale_ms(const void* const* peer_slots, void* const* peer_flags, int world,
+                                                 int rank, const int* slot_owner, int n_slots, int n_regions,
+                                                 const float* masks, long long n, float guidance, void* eps_out,
+                                                 const void* latents, void* latents_out, const void* latents_ref,
+                                                 void* latents_ref_out, float hx, float he, float cx, float cd,
+                                                 float cp, const float* d_prev, float* d_out, const float* d_prev_ref,
+                                                 float* d_out_ref, unsigned int step_id, float guidance_rescale,
+                                                 void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleMsParams p{};
+  int rc = gather_rescale_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                               eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = ms_step_args(cp, d_prev, d_out);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = ms_step_args(cp, d_prev_ref, d_out_ref);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.ms = MsStep{hx, he, cx, cd, cp, d_prev, d_out};
+  p.ms_ref = MsStep{hx, he, cx, cd, cp, d_prev_ref, d_out_ref};
   return launch_rescale<true>(p, stream);
 }

@@ -343,10 +343,20 @@ __global__ void geglu_kernel(const __half* __restrict__ proj, __half* __restrict
 // ============================================================================ region blend + CFG
 struct BlendPtrs { const __half* eps[16]; };
 
-__global__ void region_blend_kernel(const __half* __restrict__ eps_uncond, BlendPtrs ptrs,
-                                    const float* __restrict__ masks, int n_regions, long long n, float guidance,
-                                    __half* __restrict__ eps_out, const __half* __restrict__ latents,
-                                    __half* __restrict__ latents_out, float dt_sigma) {
+// step policies (rtti_internal.h): Euler, or the multistep update of MsStep
+struct EulerStep { float dt_sigma; };
+__device__ __forceinline__ void apply_step(const EulerStep& s, long long, const float* e16, float* x) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], s.dt_sigma, x[i]);
+}
+__device__ __forceinline__ void apply_step(const MsStep& s, long long v, const float* e16, float* x) { ms_step8(s, v, e16, x); }
+
+template <class Step>
+__device__ __forceinline__ void region_blend_body(const __half* __restrict__ eps_uncond, const BlendPtrs& ptrs,
+                                                  const float* __restrict__ masks, int n_regions, long long n,
+                                                  float guidance, __half* __restrict__ eps_out,
+                                                  const __half* __restrict__ latents, __half* __restrict__ latents_out,
+                                                  const Step& st) {
   const long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (v * 8 >= n) return;
   float eu[8], msum[8], et[8];
@@ -374,10 +384,23 @@ __global__ void region_blend_kernel(const __half* __restrict__ eps_uncond, Blend
     float x[8], e16[8];
     unpack8(ld8(latents + v * 8), x);
     unpack8(oh, e16);  // the scheduler consumes the fp16-rounded noise prediction
-#pragma unroll
-    for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], dt_sigma, x[i]);
+    apply_step(st, v, e16, x);
     st8(latents_out + v * 8, pack8(x));
   }
+}
+
+__global__ void region_blend_kernel(const __half* __restrict__ eps_uncond, BlendPtrs ptrs,
+                                    const float* __restrict__ masks, int n_regions, long long n, float guidance,
+                                    __half* __restrict__ eps_out, const __half* __restrict__ latents,
+                                    __half* __restrict__ latents_out, float dt_sigma) {
+  region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, EulerStep{dt_sigma});
+}
+
+__global__ void region_blend_ms_kernel(const __half* __restrict__ eps_uncond, BlendPtrs ptrs,
+                                       const float* __restrict__ masks, int n_regions, long long n, float guidance,
+                                       __half* __restrict__ eps_out, const __half* __restrict__ latents,
+                                       __half* __restrict__ latents_out, const MsStep st) {
+  region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
 }
 
 // ============================================================================ colour guidance
@@ -586,25 +609,48 @@ extern "C" int rtti_geglu_fwd(const void* proj, void* y, int rows, int inner, vo
   return ok_or_cuda();
 }
 
-extern "C" int rtti_region_blend_cfg(const void* eps_uncond, const void* const* eps_region, const float* masks,
-                                     int n_regions, long long n, float guidance, void* eps_out, const void* latents,
-                                     void* latents_out, float dt_sigma, void* stream) {
+// argument checks shared by rtti_region_blend_cfg and rtti_region_blend_cfg_ms; fills the region pointer table
+static int region_blend_args(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions,
+                             long long n, void* eps_out, const void* latents, void* latents_out, BlendPtrs& ptrs) {
   if (!eps_uncond || !eps_region || !masks || !eps_out) return RTTI_ERR_ARG;
   if (n_regions < 1 || n_regions > 16 || n < 8) return RTTI_ERR_ARG;
   if (n % 8 != 0) return RTTI_ERR_SHAPE;
   if ((latents == nullptr) != (latents_out == nullptr)) return RTTI_ERR_ARG;
-  BlendPtrs ptrs{};
   uintptr_t al = (uintptr_t)eps_uncond | (uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out;
   for (int i = 0; i < n_regions; ++i) {
     if (!eps_region[i]) return RTTI_ERR_ARG;
     ptrs.eps[i] = (const __half*)eps_region[i];
     al |= (uintptr_t)eps_region[i];
   }
-  if (al & 15) return RTTI_ERR_ALIGN;
+  return (al & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
+}
+
+extern "C" int rtti_region_blend_cfg(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                     int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                     void* latents_out, float dt_sigma, void* stream) {
+  BlendPtrs ptrs{};
+  const int rc = region_blend_args(eps_uncond, eps_region, masks, n_regions, n, eps_out, latents, latents_out, ptrs);
+  if (rc != RTTI_OK) return rc;
   const long long nv = n / 8;
   region_blend_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
       (__half*)latents_out, dt_sigma);
+  return ok_or_cuda();
+}
+
+extern "C" int rtti_region_blend_cfg_ms(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                        int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                        void* latents_out, float hx, float he, float cx, float cd, float cp,
+                                        const float* d_prev, float* d_out, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  BlendPtrs ptrs{};
+  int rc = region_blend_args(eps_uncond, eps_region, masks, n_regions, n, eps_out, latents, latents_out, ptrs);
+  if (rc == RTTI_OK) rc = ms_step_args(cp, d_prev, d_out);
+  if (rc != RTTI_OK) return rc;
+  const long long nv = n / 8;
+  region_blend_ms_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
+      (__half*)latents_out, MsStep{hx, he, cx, cd, cp, d_prev, d_out});
   return ok_or_cuda();
 }
 

@@ -57,26 +57,46 @@ __device__ __forceinline__ H8 pk8(const float* f) {
   return h;
 }
 
-__global__ void __launch_bounds__(128) gather_blend_kernel(const GatherBlendParams p) {
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    __threadfence_system();
-    asm volatile("st.release.sys.global.u32 [%0], %1;\n" ::"l"(p.peer_flags[p.rank]), "r"(p.step_id) : "memory");
-  }
-  if (threadIdx.x < p.world && threadIdx.x != p.rank) {
-    unsigned int v;
-    long long spins = 0;
-    do {
-      asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p.peer_flags[threadIdx.x]) : "memory");
-      if ((int)(v - p.step_id) < 0) {
-        __nanosleep(500);
-        if (++spins > 8000000LL) {  // ~4 s: a peer never published (crashed / diverged) — flag it, do not hang the GPU
-          p.peer_flags[p.rank][1] = 0xDEADu;
-          break;
-        }
-      }
-    } while ((int)(v - p.step_id) < 0);
-  }
+// the multistep form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory
+struct GatherBlendMsParams : GatherBlendParams {
+  MsStep ms, ms_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep update of the main / reference trajectory
+__device__ __forceinline__ void gb_step(const GatherBlendParams& p, bool, long long, const float* e16, float* x) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
+}
+__device__ __forceinline__ void gb_step(const GatherBlendMsParams& p, bool ref, long long v, const float* e16, float* x) {
+  ms_step8(ref ? p.ms_ref : p.ms, v, e16, x);
+}
+
+// steps 1 and 2: publish this rank's step, wait for every peer it reads from. A macro rather than a function: written
+// out in the kernel it compiles to the same code as before the multistep form existed (an inlined call does not).
+#define GB_PUBLISH_AND_WAIT(p) \
+  if (blockIdx.x == 0 && threadIdx.x == 0) {                                                                            \
+    __threadfence_system();                                                                                             \
+    asm volatile("st.release.sys.global.u32 [%0], %1;\n" ::"l"(p.peer_flags[p.rank]), "r"(p.step_id) : "memory");       \
+  }                                                                                                                     \
+  if (threadIdx.x < p.world && threadIdx.x != p.rank) {                                                                 \
+    unsigned int v;                                                                                                     \
+    long long spins = 0;                                                                                                \
+    do {                                                                                                                \
+      asm volatile("ld.acquire.sys.global.u32 %0, [%1];\n" : "=r"(v) : "l"(p.peer_flags[threadIdx.x]) : "memory");      \
+      if ((int)(v - p.step_id) < 0) {                                                                                   \
+        __nanosleep(500);                                                                                               \
+        if (++spins > 8000000LL) { /* ~4 s: a peer never published (crashed / diverged): flag it, do not hang */ \
+          p.peer_flags[p.rank][1] = 0xDEADu;                                                                            \
+          break;                                                                                                        \
+        }                                                                                                               \
+      }                                                                                                                 \
+    } while ((int)(v - p.step_id) < 0);                                                                                 \
+  }                                                                                                                     \
   __syncthreads();
+
+// step 3: pull the slots, blend, CFG, step
+template <class P>
+__device__ __forceinline__ void gather_blend_body(const P& p) {
   const long long v8 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (v8 * 8 >= p.n) return;
   const size_t par = (size_t)(p.step_id & 1u) * p.n_slots * p.n;
@@ -103,8 +123,7 @@ __global__ void __launch_bounds__(128) gather_blend_kernel(const GatherBlendPara
     float x[8], e16[8];
     up8(*reinterpret_cast<const H8*>(p.latents + v8 * 8), x);
     up8(oh, e16);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
+    gb_step(p, false, v8, e16, x);
     *reinterpret_cast<H8*>(p.latents_out + v8 * 8) = pk8(x);
   }
   if (p.latents_ref != nullptr) {
@@ -115,21 +134,29 @@ __global__ void __launch_bounds__(128) gather_blend_kernel(const GatherBlendPara
     for (int i = 0; i < 8; ++i) c[i] = c[i] + p.guidance * (d[i] - c[i]);
     up8(pk8(c), e16);
     up8(*reinterpret_cast<const H8*>(p.latents_ref + v8 * 8), x);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
+    gb_step(p, true, v8, e16, x);
     *reinterpret_cast<H8*>(p.latents_ref_out + v8 * 8) = pk8(x);
   }
+}
+
+__global__ void __launch_bounds__(128) gather_blend_kernel(const GatherBlendParams p) {
+  GB_PUBLISH_AND_WAIT(p);
+  gather_blend_body(p);
+}
+__global__ void __launch_bounds__(128) gather_blend_ms_kernel(const GatherBlendMsParams p) {
+  GB_PUBLISH_AND_WAIT(p);
+  gather_blend_body(p);
 }
 
 }  // namespace rtti
 
 using namespace rtti;
 
-extern "C" int rtti_gather_blend_step(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
-                                      const int* slot_owner, int n_slots, int n_regions, const float* masks,
-                                      long long n, float guidance, void* eps_out, const void* latents,
-                                      void* latents_out, const void* latents_ref, void* latents_ref_out,
-                                      float dt_sigma, unsigned int step_id, void* stream) {
+// argument checks shared by the Euler and multistep entry points; fills everything but the step
+static int gather_blend_args(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                             const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                             float guidance, void* eps_out, const void* latents, void* latents_out,
+                             const void* latents_ref, void* latents_ref_out, unsigned int step_id, GatherBlendParams& p) {
   if (!peer_slots || !peer_flags || !slot_owner || !masks || !eps_out) return RTTI_ERR_ARG;
   if (world < 1 || world > GB_MAX_WORLD || rank < 0 || rank >= world) return RTTI_ERR_ARG;
   if (n_regions < 1 || n_slots < n_regions + 1 || n_slots > GB_MAX_SLOTS || n < 8) return RTTI_ERR_ARG;
@@ -137,7 +164,6 @@ extern "C" int rtti_gather_blend_step(const void* const* peer_slots, void* const
   if ((latents == nullptr) != (latents_out == nullptr)) return RTTI_ERR_ARG;
   if ((latents_ref == nullptr) != (latents_ref_out == nullptr)) return RTTI_ERR_ARG;
   if (latents_ref != nullptr && n_slots < n_regions + 3) return RTTI_ERR_ARG;
-  GatherBlendParams p{};
   for (int r = 0; r < world; ++r) {
     if (!peer_slots[r] || !peer_flags[r]) return RTTI_ERR_ARG;
     if ((uintptr_t)peer_slots[r] & 15) return RTTI_ERR_ALIGN;
@@ -149,11 +175,48 @@ extern "C" int rtti_gather_blend_step(const void* const* peer_slots, void* const
     p.slot_owner[s] = slot_owner[s];
   }
   p.world = world; p.rank = rank; p.n_slots = n_slots; p.n_regions = n_regions; p.n = n;
-  p.guidance = guidance; p.dt_sigma = dt_sigma; p.step_id = step_id;
+  p.guidance = guidance; p.step_id = step_id;
   p.masks = masks; p.eps_out = (__half*)eps_out;
   p.latents = (const __half*)latents; p.latents_out = (__half*)latents_out;
   p.latents_ref = (const __half*)latents_ref; p.latents_ref_out = (__half*)latents_ref_out;
+  return RTTI_OK;
+}
+
+extern "C" int rtti_gather_blend_step(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                      const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                      long long n, float guidance, void* eps_out, const void* latents,
+                                      void* latents_out, const void* latents_ref, void* latents_ref_out,
+                                      float dt_sigma, unsigned int step_id, void* stream) {
+  GatherBlendParams p{};
+  const int rc = gather_blend_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                                   eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc != RTTI_OK) return rc;
+  p.dt_sigma = dt_sigma;
   const long long nv = n / 8;
   gather_blend_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+extern "C" int rtti_gather_blend_step_ms(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                         const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                         long long n, float guidance, void* eps_out, const void* latents,
+                                         void* latents_out, const void* latents_ref, void* latents_ref_out, float hx,
+                                         float he, float cx, float cd, float cp, const float* d_prev, float* d_out,
+                                         const float* d_prev_ref, float* d_out_ref, unsigned int step_id,
+                                         void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  GatherBlendMsParams p{};
+  int rc = gather_blend_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                             eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = ms_step_args(cp, d_prev, d_out);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = ms_step_args(cp, d_prev_ref, d_out_ref);
+  if (rc == RTTI_OK && (((uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out |
+                         (uintptr_t)latents_ref | (uintptr_t)latents_ref_out) & 15))
+    rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.ms = MsStep{hx, he, cx, cd, cp, d_prev, d_out};
+  p.ms_ref = MsStep{hx, he, cx, cd, cp, d_prev_ref, d_out_ref};
+  const long long nv = n / 8;
+  gather_blend_ms_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

@@ -19,6 +19,13 @@ int make_head_map(CUtensorMap* m, const void* ptr, int head_dim, int heads, int 
 
 inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// the buffers of a multistep (DDIM / DPM-Solver++) blend step: d_out required, d_prev required when cp != 0, both
+// 16-byte aligned
+inline int ms_step_args(float cp, const float* d_prev, const float* d_out) {
+  if (!d_out || (cp != 0.f && !d_prev)) return RTTI_ERR_ARG;
+  return (((uintptr_t)d_prev | (uintptr_t)d_out) & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
+}
+
 #ifdef __CUDACC__
 // GroupNorm statistics of a set of values as (count n, mean, m2 = sum of squared deviations from the mean), merged with
 // the pairwise update of Chan, Golub & LeVeque. Unlike a one-pass E[x^2] - E[x]^2 in fp32, which loses about
@@ -54,6 +61,39 @@ __device__ __forceinline__ void gn_lane_stats(const float* __restrict__ ws_bg, i
     }
 #pragma unroll
     for (int u = 0; u < 8; ++u) stats_merge(n, mean, m2, nk[u], v[u].x, v[u].y);
+  }
+}
+
+// The step policies of the blend kernels (elementwise.cu, gather_blend.cu, blend_rescale.cu): each family has one body,
+// instantiated with the Euler update (x' = x + dt_sigma * eps) or with the multistep update of DDIM / DPM-Solver++(2M)
+// in data-prediction form (schedulers.py, StepCoeffs):
+//   D  = hx * x + he * eps            written to d_out in fp32
+//   x' = cx * x + cd * D + cp * D_prev    D_prev read from d_prev only when cp != 0
+// eps is the fp16-rounded noise prediction the kernel stores, x the fp16 latents. d_prev may alias d_out: each thread
+// reads its 8 elements of d_prev before it writes the same 8 elements of d_out.
+struct MsStep {
+  float hx, he, cx, cd, cp;
+  const float* d_prev;
+  float* d_out;
+};
+
+__device__ __forceinline__ void ms_step8(const MsStep& s, long long v, const float* e16, float* x) {
+  float dp[8];
+  if (s.cp != 0.f) {
+    const float4 p0 = *reinterpret_cast<const float4*>(s.d_prev + v * 8);
+    const float4 p1 = *reinterpret_cast<const float4*>(s.d_prev + v * 8 + 4);
+    dp[0] = p0.x; dp[1] = p0.y; dp[2] = p0.z; dp[3] = p0.w; dp[4] = p1.x; dp[5] = p1.y; dp[6] = p1.z; dp[7] = p1.w;
+  }
+  float d[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) d[i] = fmaf(s.he, e16[i], s.hx * x[i]);
+  *reinterpret_cast<float4*>(s.d_out + v * 8) = make_float4(d[0], d[1], d[2], d[3]);
+  *reinterpret_cast<float4*>(s.d_out + v * 8 + 4) = make_float4(d[4], d[5], d[6], d[7]);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    float o = fmaf(s.cd, d[i], s.cx * x[i]);
+    if (s.cp != 0.f) o = fmaf(s.cp, dp[i], o);
+    x[i] = o;
   }
 }
 

@@ -220,11 +220,40 @@ def geglu(proj, out=None):
     return out
 
 
-def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0):
+class MultistepStep:
+    """The multistep (DDIM / DPM-Solver++) update of one blend call: `coeffs` (schedulers.StepCoeffs: hx, he, cx, cd, cp)
+    and the fp32 histories of D = hx x + he eps, [n] each: d_prev (read when cp != 0; may be the same tensor as d_out)
+    and d_out (written). d_prev_ref / d_out_ref: the reference-latent trajectory's (gather_blend_step only)."""
+
+    def __init__(self, coeffs, d_prev, d_out, d_prev_ref=None, d_out_ref=None):
+        self.coeffs = tuple(float(c) for c in coeffs)
+        self.d_prev, self.d_out, self.d_prev_ref, self.d_out_ref = d_prev, d_out, d_prev_ref, d_out_ref
+
+    def _check(self, n, ref):
+        pairs = [(self.d_prev, self.d_out)] + ([(self.d_prev_ref, self.d_out_ref)] if ref else [])
+        for prev, out in pairs:
+            for t, name in ((prev, "d_prev"), (out, "d_out")):
+                if t is None:
+                    if name == "d_out" or self.coeffs[4] != 0.0:
+                        raise _lib.RttiError(f"multistep blend: {name} is required")
+                    continue
+                _req(t, torch.float32, name)
+                if not t.is_contiguous() or t.numel() != n:
+                    raise _lib.RttiError(f"multistep blend: {name} must be a contiguous fp32 tensor of {n} elements")
+
+    def args(self, ref=False):
+        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(self.d_prev), _ptr(self.d_out)]
+        return a + ([_ptr(self.d_prev_ref), _ptr(self.d_out_ref)] if ref else [])
+
+
+def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0,
+                     step=None):
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
     eps_regions: list of fp16 tensors (region passes in mask order, base-prompt pass last); masks fp32 [N, n].
     guidance_rescale = phi > 0 scales eps by 1 - phi + phi std(eps_t) / std(eps) before it is stored and stepped
-    (rtti_region_blend_cfg_rescale); phi == 0 runs rtti_region_blend_cfg."""
+    (rtti_region_blend_cfg_rescale); phi == 0 runs rtti_region_blend_cfg.
+    step: a MultistepStep — the latents (required then) take the DDIM / DPM-Solver++ update instead of the Euler one
+    (rtti_region_blend_cfg_ms / rtti_region_blend_cfg_rescale_ms; dt_sigma is not used)."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -235,7 +264,20 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    if guidance_rescale == 0.0:
+    if step is not None:
+        if latents is None:
+            raise _lib.RttiError("region_blend_cfg: a multistep step needs the latents")
+        step._check(n, False)
+        if guidance_rescale == 0.0:
+            rc = lib.rtti_region_blend_cfg_ms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
+                                              _ptr(latents), _ptr(lat_out), *step.args(), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_ms")
+        else:
+            rc = lib.rtti_region_blend_cfg_rescale_ms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                      _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
+                                                      float(guidance_rescale), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_rescale_ms")
+    elif guidance_rescale == 0.0:
         rc = lib.rtti_region_blend_cfg(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
                                        _ptr(latents), _ptr(lat_out), float(dt_sigma), _stream())
         _lib.check(rc, "rtti_region_blend_cfg")
@@ -312,9 +354,11 @@ def predict_x0(x_t, eps, alpha):
 
 
 def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_regions, masks, guidance, latents, latents_ref,
-                      dt_sigma, step_id, guidance_rescale=0.0):
+                      dt_sigma, step_id, guidance_rescale=0.0, step=None):
     """Fused all-gather + blend + CFG + Euler over NVLink peer memory (rtti_gather_blend_step; with
     guidance_rescale > 0 rtti_gather_blend_step_rescale, which also rescales the reference-latent pair).
+    step: a MultistepStep (with d_prev_ref / d_out_ref when latents_ref is given) — the DDIM / DPM-Solver++ update
+    instead of the Euler one (rtti_gather_blend_step_ms / rtti_gather_blend_step_rescale_ms).
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
@@ -325,7 +369,17 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    if guidance_rescale == 0.0:
+    if step is not None:
+        step._check(n, latents_ref is not None)
+        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
+                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
+        args += step.args(ref=True) + [int(step_id)]
+        if guidance_rescale == 0.0:
+            _lib.check(lib.rtti_gather_blend_step_ms(*args, _stream()), "rtti_gather_blend_step_ms")
+        else:
+            _lib.check(lib.rtti_gather_blend_step_rescale_ms(*args, float(guidance_rescale), _stream()),
+                       "rtti_gather_blend_step_rescale_ms")
+    elif guidance_rescale == 0.0:
         rc = lib.rtti_gather_blend_step(slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions,
                                         _ptr(masks), n, float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out),
                                         _ptr(latents_ref), _ptr(ref_out), float(dt_sigma), int(step_id), _stream())

@@ -6,6 +6,10 @@ Public surface kept: `RegionDiffusion(device)`, `produce_attn_maps`, `produce_la
 models/region_diffusion.py:86-174 (including its differences from the SDXL loop: no scale_model_input,
 joint stepping on every step when injecting, `i == int(...)` background flag, and the self-attention
 capture that overwrites instead of accumulating, :423), executed as one batched UNet call per step.
+
+`.scheduler` is PLMS (PNDMScheduler) by default and steps on the host; DDIMScheduler and DPMSolverMultistepScheduler
+(schedulers.py) step inside the fused blend kernels (rtti_region_blend_cfg_ms), with one fp32 history of the x0
+prediction per trajectory.
 """
 import math
 from typing import Optional
@@ -15,7 +19,7 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers, SelfAttentionLayers
-from .schedulers import PNDMScheduler
+from .schedulers import MULTISTEP_SCHEDULERS, PNDMScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -135,6 +139,10 @@ class RegionDiffusion:
             word_pos = font_size = None
         kv_caches = {}
         n_t = len(timesteps)
+        multistep = isinstance(self.scheduler, MULTISTEP_SCHEDULERS)
+        if multistep:   # one x0-prediction history per trajectory (both are stepped on every step)
+            d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev)
+            d_hist_ref = torch.empty_like(d_hist) if inject else None
         for i, t in enumerate(timesteps):
             feat_inject_step = bool(int(t) > (1 - inject_selfattn) * 1000)                                   # :104
             background_inject_step = (i == int(inject_background * n_t)) and inject_background > 0           # :105
@@ -154,14 +162,25 @@ class RegionDiffusion:
             eps = plan.gather(eps_local, local, feat_inject_step)
             regions = [eps[kind[f"E{j}"]:kind[f"E{j}"] + 1].contiguous() for j in range(N - 1)]
             regions.append(eps[kind["B"]:kind["B"] + 1].contiguous())
-            noise_pred = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks, guidance_scale)  # :119-132
-            if inject:                                                                                      # :134-143
-                ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
-                                           [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale)
-                both = self.scheduler.step(torch.cat([noise_pred, ref]), t, torch.cat([latents, latents_ref]))["prev_sample"]
-                latents, latents_ref = [c.to(torch.float16) for c in torch.chunk(both, 2, dim=0)]
+            if multistep:
+                c = self.scheduler.step_coeffs(i)
+                noise_pred, latents = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks,
+                                                           guidance_scale, latents=latents.contiguous(),
+                                                           step=ops.MultistepStep(c, d_hist, d_hist))
+                if inject:
+                    _, latents_ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
+                                                          [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale,
+                                                          latents=latents_ref.contiguous(),
+                                                          step=ops.MultistepStep(c, d_hist_ref, d_hist_ref))
             else:
-                latents = self.scheduler.step(noise_pred, t, latents)["prev_sample"].to(torch.float16)
+                noise_pred = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks, guidance_scale)  # :119-132
+                if inject:                                                                                  # :134-143
+                    ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
+                                               [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale)
+                    both = self.scheduler.step(torch.cat([noise_pred, ref]), t, torch.cat([latents, latents_ref]))["prev_sample"]
+                    latents, latents_ref = [c.to(torch.float16) for c in torch.chunk(both, 2, dim=0)]
+                else:
+                    latents = self.scheduler.step(noise_pred, t, latents)["prev_sample"].to(torch.float16)
             if use_guidance and int(t) < tfd["guidance_start_step"]:                                        # :151
                 latents = self._color_guidance(latents, noise_pred, t, tfd)
             if background_inject_step:                                                                       # :171-173
@@ -184,10 +203,17 @@ class RegionDiffusion:
         self.scheduler.set_timesteps(num_inference_steps)
         kv = CrossKVCache()
         ones = torch.ones(1, latents[0].numel(), dtype=torch.float32, device=dev)
-        for t in self.scheduler.timesteps:
+        multistep = isinstance(self.scheduler, MULTISTEP_SCHEDULERS)
+        d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev) if multistep else None
+        for i, t in enumerate(self.scheduler.timesteps):
             x = latents.expand(2, -1, -1, -1)
             ctrl = RegionControl(capture=self._capture, capture_row=1, kv_cache=kv)
             eps = self.unet(x, t, ctx, None, ctrl)["sample"]
+            if multistep:
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=latents.contiguous(),
+                                                  step=ops.MultistepStep(self.scheduler.step_coeffs(i), d_hist, d_hist))
+                continue
             noise_pred = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale)
             latents = self.scheduler.step(noise_pred, t, latents)["prev_sample"].to(torch.float16)
         self._last_latents = latents

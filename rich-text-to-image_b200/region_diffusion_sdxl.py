@@ -7,8 +7,9 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
   * the 2 + 2*inject + (N-1) UNet passes of a step (uncond, base+font-size, reference uncond, reference
     base, N-1 regions; :787-821) run as ONE batched UNet call — they share the timestep and, up to the
     reference latent, the input; the hook choreography becomes a RegionControl;
-  * region blend + CFG (+ guidance rescale) + Euler update is one kernel (rtti_region_blend_cfg, or
-    rtti_region_blend_cfg_rescale with guidance_rescale > 0); colour-guidance loss fwd/bwd,
+  * region blend + CFG (+ guidance rescale) + scheduler update is one kernel (rtti_region_blend_cfg, or
+    rtti_region_blend_cfg_rescale with guidance_rescale > 0; their "_ms" forms for DDIM / DPM-Solver++(2M), which
+    keep one fp32 history of the x0 prediction per trajectory); colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
     per-pass noise predictions are all-gathered before the (replicated, deterministic) blend.
@@ -21,7 +22,7 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
-from .schedulers import EulerDiscreteScheduler
+from .schedulers import MULTISTEP_SCHEDULERS, DDIMScheduler, EulerDiscreteScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -29,6 +30,17 @@ from .vae import AutoencoderKLDecoder, VAEConfig
 def _rescale_phi(guidance_scale, guidance_rescale):
     """The guidance rescale in effect: the reference applies it only with classifier-free guidance on (:903)."""
     return float(guidance_rescale) if guidance_scale > 1.0 and guidance_rescale > 0.0 else 0.0
+
+
+def _is_multistep(scheduler):
+    """False: EulerDiscreteScheduler (the fused Euler update); True: DDIMScheduler / DPMSolverMultistepScheduler (the
+    fused multistep update, step_coeffs). Any other scheduler has no fused update here."""
+    if isinstance(scheduler, EulerDiscreteScheduler):
+        return False
+    if isinstance(scheduler, MULTISTEP_SCHEDULERS):
+        return True
+    raise TypeError(f"RegionDiffusionXL: unsupported scheduler {type(scheduler).__name__}; supported: "
+                    "EulerDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler (rtti_b200.schedulers)")
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -192,7 +204,16 @@ class RegionDiffusionXL:
         """Signature of models/region_diffusion_sdxl.py:556-587. `prompt` is the list of region prompts with the
         base prompt last (sample.py:107); embeddings may be passed instead of text. `guidance_rescale` (applied when
         guidance_scale > 1) rescales the CFG prediction as diffusers' rescale_noise_cfg in both passes; the reference
-        implements it for the plain pass only (:903-905) and raises NotImplementedError in the rich-text pass (:827-830)."""
+        implements it for the plain pass only (:903-905) and raises NotImplementedError in the rich-text pass (:827-830).
+        `self.scheduler` may be EulerDiscreteScheduler, DDIMScheduler or DPMSolverMultistepScheduler (schedulers.py);
+        `eta` > 0 (stochastic DDIM, which the reference's plain pass forwards to DDIM) is not implemented.
+        With a multistep scheduler the rich-text pass keeps one history per trajectory: where the reference steps the
+        reference latents jointly with the main latents only on a prefix of the steps (inject_selfattn = 0,
+        0 < inject_background < 1, :831-846) and then steps the main latents alone, the main latents keep their own
+        history here instead of continuing a batch-2 one."""
+        multistep = _is_multistep(self.scheduler)
+        if multistep and eta > 0 and not run_rich_text and isinstance(self.scheduler, DDIMScheduler):
+            raise NotImplementedError("RegionDiffusionXL: DDIM with eta > 0 is not implemented")
         height = height or self.default_sample_size * self.vae_scale_factor
         width = width or self.default_sample_size * self.vae_scale_factor
         original_size = original_size or (height, width)
@@ -233,23 +254,34 @@ class RegionDiffusionXL:
     def _plain_loop(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps,
                     guidance_rescale=0.0):
         """:879-914 — CFG batch [uncond, cond]; with capture armed the attention kernels accumulate the maps.
-        guidance_rescale rescales the CFG prediction inside the blend kernel (:903-905)."""
+        guidance_rescale rescales the CFG prediction inside the blend kernel (:903-905). A multistep scheduler: the UNet
+        sees the latents unscaled and the blend kernel takes the step_coeffs(i) update."""
         phi = _rescale_phi(guidance_scale, guidance_rescale)
         ctx2 = torch.cat([ctx[:1], ctx[-1:]])
         pooled2 = torch.cat([pooled[:1], pooled[-1:]])
         kv = CrossKVCache()
         ones = None
+        multistep = _is_multistep(self.scheduler)
+        d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=latents.device) if multistep else None
         for i, t in enumerate(timesteps):
-            sigma = self.scheduler.sigma(t)
-            x = (latents / math.sqrt(sigma * sigma + 1.0)).expand(2, -1, -1, -1)
+            if multistep:
+                x = latents.expand(2, -1, -1, -1)
+            else:
+                sigma = self.scheduler.sigma(t)
+                x = (latents / math.sqrt(sigma * sigma + 1.0)).expand(2, -1, -1, -1)
             ctrl = RegionControl(capture=self._capture, capture_row=1, kv_cache=kv)
             eps = self.unet(x, t, ctx2, {"text_embeds": pooled2, "time_ids": time_ids}, ctrl)["sample"]
             n = eps[0].numel()
             if ones is None:
                 ones = torch.ones(1, n, dtype=torch.float32, device=eps.device)
-            _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                              latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
-                                              guidance_rescale=phi)
+            if multistep:
+                step = ops.MultistepStep(self.scheduler.step_coeffs(i), d_hist, d_hist)
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=latents.contiguous(), guidance_rescale=phi, step=step)
+            else:
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
+                                                  guidance_rescale=phi)
             if callback is not None and i % callback_steps == 0:
                 callback(i, t, latents)
         return latents
@@ -301,6 +333,11 @@ class RegionDiffusionXL:
         st.kv_caches = {}
         st.graphs = {}
         st.noise_pred = None
+        # multistep schedulers: one fp32 history of the x0 prediction per trajectory (main, reference)
+        st.multistep = _is_multistep(self.scheduler)
+        n = latents.numel()
+        st.d_hist = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep else None
+        st.d_hist_ref = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep and inject else None
         return st
 
     def _unet_pass(self, st, x, t, local, feat_inject_step):
@@ -395,8 +432,11 @@ class RegionDiffusionXL:
         passes, kind, plan, N = st.passes, st.kind, st.plan, st.N
         feat_inject_step = bool(float(t) > (1 - st.inject_selfattn) * 1000)            # :782
         background_inject_step = i < st.inject_background * st.n_t                      # :783
-        sigma = self.scheduler.sigma(t)
-        scale = 1.0 / math.sqrt(sigma * sigma + 1.0)                                    # :784
+        if st.multistep:   # scale_model_input is the identity
+            scale = None
+        else:
+            sigma = self.scheduler.sigma(t)
+            scale = 1.0 / math.sqrt(sigma * sigma + 1.0)                                # :784
         if feat_inject_step and st.inject:
             self._remote_qk(st, st.latents)   # collective on first use: every rank of the group, also those without passes
         local = plan.local_passes(feat_inject_step)
@@ -405,7 +445,9 @@ class RegionDiffusionXL:
             ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
             ev[0].record()
         if local:
-            x = torch.cat([(st.latents_ref if passes[p]["ref"] else st.latents) for p in local]) * scale
+            x = torch.cat([(st.latents_ref if passes[p]["ref"] else st.latents) for p in local])
+            if scale is not None:
+                x = x * scale
             eps_local = self._unet_pass(st, x, t, local, feat_inject_step)
         else:   # more ranks than passes on this step: this rank only takes part in the exchange
             eps_local = st.latents.new_empty((0,) + tuple(st.latents.shape[1:]))
@@ -415,7 +457,13 @@ class RegionDiffusionXL:
                 rq.end_pass()
         if pe is not None:
             ev[1].record()
-        dt = self.scheduler.dt(t)
+        if st.multistep:
+            c = self.scheduler.step_coeffs(i)
+            dt = 0.0
+            step = ops.MultistepStep(c, st.d_hist, st.d_hist, st.d_hist_ref, st.d_hist_ref)
+        else:
+            dt = self.scheduler.dt(t)
+            step = None
         step_ref = st.inject and (st.inject_selfattn > 0 or background_inject_step)                       # :830-841
         ex = None
         if plan.world > 1 and self.fused_exchange:
@@ -435,7 +483,7 @@ class RegionDiffusionXL:
             st.noise_pred, st.latents, ref_out = ops.gather_blend_step(
                 ex.slot_ptrs, ex.flag_ptrs, ex.rank, ex.slot_owner(owner), N, st.masks, st.guidance_scale,
                 st.latents.contiguous(), st.latents_ref.contiguous() if step_ref else None, dt, sid,
-                guidance_rescale=st.guidance_rescale)
+                guidance_rescale=st.guidance_rescale, step=step)
             if step_ref:
                 st.latents_ref = ref_out
         else:
@@ -444,11 +492,13 @@ class RegionDiffusionXL:
             regions = [one(f"E{j}") for j in range(N - 1)] + [one("B")]
             st.noise_pred, st.latents = ops.region_blend_cfg(one("A"), regions, st.masks, st.guidance_scale,
                                                               latents=st.latents.contiguous(), dt_sigma=dt,
-                                                              guidance_rescale=st.guidance_rescale)   # :810-830, :845
+                                                              guidance_rescale=st.guidance_rescale,
+                                                              step=ops.MultistepStep(c, st.d_hist, st.d_hist) if step else None)  # :810-830
             if step_ref:
                 _, st.latents_ref = ops.region_blend_cfg(one("C"), [one("D")], st.ones, st.guidance_scale,
                                                          latents=st.latents_ref.contiguous(), dt_sigma=dt,
-                                                         guidance_rescale=st.guidance_rescale)
+                                                         guidance_rescale=st.guidance_rescale,
+                                                         step=ops.MultistepStep(c, st.d_hist_ref, st.d_hist_ref) if step else None)
         if pe is not None:
             ev[2].record()
         if st.use_guidance and float(t) < st.tfd["guidance_start_step"]:                                  # :849

@@ -5,7 +5,14 @@ models/region_diffusion.py:35-37; EulerDiscrete for SDXL, models/region_diffusio
 sources are not part of the reference tree, so the published algorithms are restated here; only the
 calls the reference makes are provided: set_timesteps / timesteps / scale_model_input / step /
 init_noise_sigma / alphas_cumprod.  All state lives on the sampling device; `step` never synchronises.
+
+DDIMScheduler and DPMSolverMultistepScheduler (below) are the schedulers a diffusers user swaps in
+(`model.scheduler = DPMSolverMultistepScheduler(...)`); the samplers run them through the fused blend kernels with
+the per-step coefficients of `step_coeffs(i)`.
 """
+import math
+from typing import NamedTuple
+
 import numpy as np
 import torch
 
@@ -15,12 +22,19 @@ def _alphas_cumprod(beta_start, beta_end, n):
     return torch.cumprod(1.0 - betas, dim=0)
 
 
+class _Config(dict):
+    """Scheduler configuration: a dict with attribute access (diffusers' scheduler.config)."""
+    __getattr__ = dict.get
+
+
 class EulerDiscreteScheduler:
     """EulerDiscrete, epsilon prediction, scaled-linear betas, `leading` spacing, steps_offset=1 (SDXL config)."""
     order = 1
 
     def __init__(self, beta_start=0.00085, beta_end=0.012, num_train_timesteps=1000, steps_offset=1):
         self.num_train_timesteps, self.steps_offset = num_train_timesteps, steps_offset
+        self.config = _Config(beta_start=beta_start, beta_end=beta_end, num_train_timesteps=num_train_timesteps,
+                              steps_offset=steps_offset, beta_schedule="scaled_linear")
         self.alphas_cumprod = _alphas_cumprod(beta_start, beta_end, num_train_timesteps)  # host copy (predict_x0)
         self._sig_all = (((1 - self.alphas_cumprod) / self.alphas_cumprod) ** 0.5).numpy()
         self.sigmas_host = np.concatenate([self._sig_all[::-1], [0.0]]).astype(np.float32)
@@ -65,6 +79,8 @@ class PNDMScheduler:
 
     def __init__(self, beta_start=0.00085, beta_end=0.012, num_train_timesteps=1000, steps_offset=1):
         self.num_train_timesteps, self.steps_offset = num_train_timesteps, steps_offset
+        self.config = _Config(beta_start=beta_start, beta_end=beta_end, num_train_timesteps=num_train_timesteps,
+                              steps_offset=steps_offset, beta_schedule="scaled_linear")
         self.alphas_cumprod = _alphas_cumprod(beta_start, beta_end, num_train_timesteps)
         self.final_alpha_cumprod = float(self.alphas_cumprod[0])
         self.init_noise_sigma = 1.0
@@ -113,3 +129,154 @@ class PNDMScheduler:
         denom = a_t * b_prev ** 0.5 + (a_t * b_t * a_prev) ** 0.5
         self.counter += 1
         return {"prev_sample": coeff * sample - (a_prev - a_t) * model_output / denom}
+
+
+# ---------------------------------------------------------------------------------------------------- multistep
+class StepCoeffs(NamedTuple):
+    """One step of DDIM / DPM-Solver++(2M) in data-prediction form (float64, host):
+        D  = hx * x + he * eps                      (x0 prediction, hx = 1/alpha_t, he = -sigma_t/alpha_t)
+        x' = cx * x + cd * D + cp * D_prev          (D_prev: the D of the previous step; cp = 0 on first-order steps)
+    The blend kernels' multistep entry points (rtti_*_ms) evaluate exactly this with eps = the fp16-rounded prediction."""
+    hx: float
+    he: float
+    cx: float
+    cd: float
+    cp: float
+
+
+class _MultistepBase:
+    """Shared VP-space conventions of DDIMScheduler and DPMSolverMultistepScheduler: scaled-linear betas, epsilon
+    prediction, init_noise_sigma = 1, scale_model_input = identity (the UNet sees the latents unscaled),
+    alphas_cumprod = the same host fp32 tensor as the other schedulers (colour guidance's predict_x0), host int64
+    timesteps. Write a_t = alphas_cumprod[t], alpha_t = sqrt(a_t), sigma_t = sqrt(1 - a_t),
+    lambda_t = log alpha_t - log sigma_t."""
+    order = 1
+    init_noise_sigma = 1.0
+    _unsupported = {}  # keyword -> the only value this restatement implements
+
+    def __init__(self, **kw):
+        for k, v in kw.items():
+            if k in self._unsupported and v != self._unsupported[k]:
+                raise NotImplementedError(f"{type(self).__name__}: {k}={v!r} is not supported "
+                                          f"(only {k}={self._unsupported[k]!r})")
+        cfg = dict(self._defaults)
+        unknown = set(kw) - set(cfg)
+        if unknown:
+            raise TypeError(f"{type(self).__name__}: unexpected keyword arguments {sorted(unknown)}")
+        cfg.update(kw)
+        if cfg["beta_schedule"] != "scaled_linear":
+            raise NotImplementedError(f"{type(self).__name__}: beta_schedule={cfg['beta_schedule']!r} is not supported")
+        self.config = _Config(cfg)
+        self.num_train_timesteps = int(cfg["num_train_timesteps"])
+        self.alphas_cumprod = _alphas_cumprod(cfg["beta_start"], cfg["beta_end"], self.num_train_timesteps)
+        ac = self.alphas_cumprod.double().numpy()
+        self._alpha, self._sigma = np.sqrt(ac), np.sqrt(1.0 - ac)
+        self._lambda = np.log(self._alpha) - np.log(self._sigma)
+        self.timesteps = None
+        self.num_inference_steps = None
+        self._d_prev = None
+
+    @classmethod
+    def from_config(cls, config, **kw):
+        """`config`: a dict, or any scheduler of this package (its `.config`); keys this class does not take are dropped,
+        as diffusers' from_config does."""
+        cfg = dict(config if isinstance(config, dict) else config.config)
+        cfg.update(kw)
+        return cls(**{k: v for k, v in cfg.items() if k in cls._defaults})
+
+    def scale_model_input(self, sample, timestep=None):
+        return sample
+
+    def index_of(self, timestep):
+        return int(np.nonzero(self.timesteps_host == int(timestep))[0][0])
+
+    def _first_order(self, t, s):
+        """DPM-Solver-1 (= DDIM, eta 0) from timestep t to timestep s: (hx, he, cx, cd, h)."""
+        h = float(self._lambda[s] - self._lambda[t])
+        a_t, s_t, a_s, s_s = (float(v) for v in (self._alpha[t], self._sigma[t], self._alpha[s], self._sigma[s]))
+        return 1.0 / a_t, -s_t / a_t, s_s / s_t, -a_s * math.expm1(-h), h
+
+    def step(self, model_output, timestep, sample, eta=0.0, return_dict=True, **kw):
+        """Stateful torch form of step_coeffs (the samplers use the fused kernels instead): keeps D of the last step."""
+        if eta:
+            raise NotImplementedError(f"{type(self).__name__}: eta > 0 is not supported")
+        c = self.step_coeffs(self.index_of(timestep))
+        x, e = sample.float(), model_output.float()
+        d = c.hx * x + c.he * e
+        prev = c.cx * x + c.cd * d
+        if c.cp != 0.0:
+            prev = prev + c.cp * self._d_prev
+        self._d_prev = d
+        prev = prev.to(sample.dtype)
+        return {"prev_sample": prev} if return_dict else (prev,)
+
+
+class DDIMScheduler(_MultistepBase):
+    """DDIM, eta = 0, with the SD1.5 / SDXL scheduler configs (steps_offset=1, set_alpha_to_one=False,
+    clip_sample=False), restating diffusers 0.18.2 (`schedulers/scheduling_ddim.py`). PARITY UNPINNED: that source is not
+    available here; the conventions below are the definition.
+      timesteps = arange(N) * (1000 // N), reversed, + steps_offset
+      prev = t - 1000 // N;  a_prev = alphas_cumprod[prev], or alphas_cumprod[0] if prev < 0
+      x' = sqrt(a_prev) * x0_hat + sqrt(1 - a_prev) * eps,   x0_hat = (x - sigma_t eps) / alpha_t
+    which is DPM-Solver-1: cx = sigma_prev / sigma_t, cd = -alpha_prev * expm1(-h), cp = 0 (step_coeffs)."""
+    _defaults = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                     trained_betas=None, clip_sample=False, set_alpha_to_one=False, steps_offset=1,
+                     prediction_type="epsilon", thresholding=False, dynamic_thresholding_ratio=0.995,
+                     clip_sample_range=1.0, sample_max_value=1.0, timestep_spacing="leading")
+    _unsupported = dict(trained_betas=None, clip_sample=False, set_alpha_to_one=False, prediction_type="epsilon",
+                        thresholding=False, timestep_spacing="leading")
+
+    def set_timesteps(self, num_inference_steps, device=None):
+        self.num_inference_steps = num_inference_steps
+        ratio = self.num_train_timesteps // num_inference_steps
+        ts = (np.arange(0, num_inference_steps) * ratio).round()[::-1].astype(np.int64) + int(self.config.steps_offset)
+        self.timesteps_host = ts.copy()
+        self.timesteps = torch.from_numpy(self.timesteps_host.copy())
+        self._d_prev = None
+
+    def step_coeffs(self, i):
+        t = int(self.timesteps_host[i])
+        prev = t - self.num_train_timesteps // self.num_inference_steps
+        hx, he, cx, cd, _ = self._first_order(t, max(prev, 0))   # set_alpha_to_one=False: prev < 0 lands on index 0
+        return StepCoeffs(hx, he, cx, cd, 0.0)
+
+
+class DPMSolverMultistepScheduler(_MultistepBase):
+    """DPM-Solver++(2M): algorithm_type="dpmsolver++", solver_order=2, solver_type="midpoint", lower_order_final=True,
+    no Karras sigmas, epsilon prediction — the defaults of diffusers 0.18.2 (`schedulers/scheduling_dpmsolver_multistep.py`),
+    restated. PARITY UNPINNED: that source is not available here; the conventions below are the definition.
+      timesteps = linspace(0, 999, N+1).round()[::-1][:-1], duplicates removed in order (N may shrink at N ~ 1000)
+      step i: t = ts[i] -> s = ts[i+1] (s = 0 on the last step), h = lambda_s - lambda_t, D_i = x0_hat at step i
+      first order (step 0, and the last step when len(ts) < 15): x' = (sigma_s/sigma_t) x - alpha_s expm1(-h) D_i
+      otherwise, r = (lambda_t - lambda_{t_prev}) / h:
+                  x' = (sigma_s/sigma_t) x - alpha_s expm1(-h) (D_i + (D_i - D_{i-1}) / (2r))"""
+    _defaults = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                     trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                     dynamic_thresholding_ratio=0.995, sample_max_value=1.0, algorithm_type="dpmsolver++",
+                     solver_type="midpoint", lower_order_final=True, use_karras_sigmas=False, lambda_min_clipped=-float("inf"),
+                     variance_type=None, steps_offset=1, set_alpha_to_one=False, clip_sample=False,
+                     timestep_spacing="linspace")
+    _unsupported = dict(trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                        algorithm_type="dpmsolver++", solver_type="midpoint", use_karras_sigmas=False,
+                        lambda_min_clipped=-float("inf"), variance_type=None, timestep_spacing="linspace")
+
+    def set_timesteps(self, num_inference_steps, device=None):
+        ts = np.linspace(0, self.num_train_timesteps - 1, num_inference_steps + 1).round()[::-1][:-1].astype(np.int64)
+        _, first = np.unique(ts, return_index=True)
+        self.timesteps_host = ts[np.sort(first)].copy()
+        self.timesteps = torch.from_numpy(self.timesteps_host.copy())
+        self.num_inference_steps = len(self.timesteps_host)
+        self._d_prev = None
+
+    def step_coeffs(self, i):
+        ts, n = self.timesteps_host, len(self.timesteps_host)
+        t = int(ts[i])
+        s = 0 if i == n - 1 else int(ts[i + 1])
+        hx, he, cx, cd, h = self._first_order(t, s)
+        if i == 0 or (i == n - 1 and self.config.lower_order_final and n < 15):
+            return StepCoeffs(hx, he, cx, cd, 0.0)
+        r = (self._lambda[t] - self._lambda[int(ts[i - 1])]) / h
+        return StepCoeffs(hx, he, cx, cd * (1.0 + 0.5 / r), -cd * 0.5 / r)
+
+
+MULTISTEP_SCHEDULERS = (DDIMScheduler, DPMSolverMultistepScheduler)
