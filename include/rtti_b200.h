@@ -157,6 +157,22 @@ int rtti_region_blend_cfg_rescale_ms(const void* eps_uncond, const void* const* 
                                      void* latents_out, float hx, float he, float cx, float cd, float cp,
                                      const float* d_prev, float* d_out, float guidance_rescale, void* stream);
 
+/* Ancestral forms ("_anc") of the blend entry points, for Euler Ancestral (rich-text-to-image_b200/schedulers.py,
+ * EulerAncestralDiscreteScheduler.ancestral_coeffs). The blend, CFG and rescale arithmetic is that of the Euler form;
+ * the update of the latents is, in fp32,
+ *   x' = fma(z, s_up, fma(eps, dt_sigma, x))    (dt_sigma = sigma_down - sigma; x' rounded to fp16)
+ * with x the fp16 latents, eps the fp16-rounded noise prediction written to eps_out and z[n] the fp16 noise of the step,
+ * read only when s_up != 0 (with s_up == 0 the result equals the Euler form's with the same dt_sigma, bit for bit).
+ * latents and latents_out are required; z is required when s_up != 0 and must be 16-byte aligned. The other checks are
+ * those of the Euler form; on any error nothing is launched. */
+int rtti_region_blend_cfg_anc(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions,
+                              long long n, float guidance, void* eps_out, const void* latents, void* latents_out,
+                              float dt_sigma, float s_up, const void* z, void* stream);
+int rtti_region_blend_cfg_rescale_anc(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                      int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                      void* latents_out, float dt_sigma, float s_up, const void* z,
+                                      float guidance_rescale, void* stream);
+
 /* Colour-guidance loss forward + analytic backward w.r.t. the VAE decoder output.
  * Replaces models/region_diffusion_sdxl.py:857-865 (clamp, masked mean RGB, MSE*100, autograd of those).
  *   decoded [3, hw] fp32 (VAE output before /2+0.5), masks [n_colors, hw] fp32 (channel 0 of
@@ -259,6 +275,21 @@ int rtti_gather_blend_step_rescale_ms(const void* const* peer_slots, void* const
                                       float he, float cx, float cd, float cp, const float* d_prev, float* d_out,
                                       const float* d_prev_ref, float* d_out_ref, unsigned int step_id,
                                       float guidance_rescale, void* stream);
+
+/* Ancestral forms of rtti_gather_blend_step / rtti_gather_blend_step_rescale (the update of rtti_region_blend_cfg_anc).
+ * Both trajectories take the same dt_sigma and s_up; the reference latents take their own noise z_ref[n], required
+ * (16-byte aligned) when latents_ref is given and s_up != 0. Same protocol and slot layout as the Euler forms. */
+int rtti_gather_blend_step_anc(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                               const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                               float guidance, void* eps_out, const void* latents, void* latents_out,
+                               const void* latents_ref, void* latents_ref_out, float dt_sigma, float s_up,
+                               const void* z, const void* z_ref, unsigned int step_id, void* stream);
+int rtti_gather_blend_step_rescale_anc(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                       const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                       long long n, float guidance, void* eps_out, const void* latents,
+                                       void* latents_out, const void* latents_ref, void* latents_ref_out,
+                                       float dt_sigma, float s_up, const void* z, const void* z_ref,
+                                       unsigned int step_id, float guidance_rescale, void* stream);
 
 /* Stripe-parallel colour guidance (multi-GPU; new relative to the single-GPU reference, which back-propagates
  * through the batch-1 VAE decoder on one device: models/region_diffusion_sdxl.py:849-867). Every activation of

@@ -59,8 +59,15 @@ struct RescaleMsParams : RescaleParams {
   MsStep ms, ms_ref;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep update of the main (REF false) / reference
-// (REF true) trajectory
+// the ancestral form: the parameters of the Euler form + the noise of each trajectory
+struct RescaleAncParams : RescaleParams {
+  float s_up;
+  const __half* z;
+  const __half* z_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral update of the main (REF false) /
+// reference (REF true) trajectory
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleParams& p, long long, const float* e16, float* x) {
 #pragma unroll
@@ -69,6 +76,10 @@ __device__ __forceinline__ void rs_step(const RescaleParams& p, long long, const
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleMsParams& p, long long v, const float* e16, float* x) {
   ms_step8(REF ? p.ms_ref : p.ms, v, e16, x);
+}
+template <bool REF>
+__device__ __forceinline__ void rs_step(const RescaleAncParams& p, long long v, const float* e16, float* x) {
+  anc_step8(AncStep{p.dt_sigma, p.s_up, REF ? p.z_ref : p.z}, v, e16, x);
 }
 
 // (count, mean, m2) of eps_text and of eps_cfg over the same elements
@@ -257,6 +268,22 @@ __global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
   blend_rescale_body<PEER>(p, cfg_s, sm);
 }
 
+template <bool PEER>
+__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
+    blend_rescale_anc_kernel(const __grid_constant__ RescaleAncParams p) {
+  extern __shared__ float4 cfg_s[];
+  __shared__ RescaleSmem sm;
+  blend_rescale_body<PEER>(p, cfg_s, sm);
+}
+
+// the kernel of each parameter type
+template <bool PEER>
+const void* rescale_kernel(const RescaleParams&) { return (const void*)blend_rescale_kernel<PEER>; }
+template <bool PEER>
+const void* rescale_kernel(const RescaleMsParams&) { return (const void*)blend_rescale_ms_kernel<PEER>; }
+template <bool PEER>
+const void* rescale_kernel(const RescaleAncParams&) { return (const void*)blend_rescale_anc_kernel<PEER>; }
+
 // threads per CTA and vectors per thread: a function of n only
 void rescale_plan(long long n, int& threads, int& vpt) {
   const long long nv = n / 8, per_cta = (nv + RS_CL - 1) / RS_CL;
@@ -271,14 +298,14 @@ void rescale_plan(long long n, int& threads, int& vpt) {
 
 template <bool PEER, class P>
 int launch_rescale(P& p, void* stream) {
-  constexpr bool MS = !std::is_same<P, RescaleParams>::value;
-  static const bool configured =
-      cudaFuncSetAttribute(MS ? (const void*)blend_rescale_ms_kernel<PEER> : (const void*)blend_rescale_kernel<PEER>,
-                           cudaFuncAttributeMaxDynamicSharedMemorySize, RS_SMEM) == cudaSuccess;
+  static const bool configured = cudaFuncSetAttribute(rescale_kernel<PEER>(p), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                      RS_SMEM) == cudaSuccess;
   if (!configured) return RTTI_ERR_CUDA;
   rescale_plan(p.n, p.threads, p.vpt);
-  if constexpr (MS)
+  if constexpr (std::is_same<P, RescaleMsParams>::value)
     blend_rescale_ms_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
+  else if constexpr (std::is_same<P, RescaleAncParams>::value)
+    blend_rescale_anc_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else
     blend_rescale_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
@@ -367,6 +394,20 @@ extern "C" int rtti_region_blend_cfg_rescale_ms(const void* eps_uncond, const vo
   return launch_rescale<false>(p, stream);
 }
 
+extern "C" int rtti_region_blend_cfg_rescale_anc(const void* eps_uncond, const void* const* eps_region,
+                                                 const float* masks, int n_regions, long long n, float guidance,
+                                                 void* eps_out, const void* latents, void* latents_out, float dt_sigma,
+                                                 float s_up, const void* z, float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleAncParams p{};
+  int rc = rescale_args(eps_uncond, eps_region, masks, n_regions, n, guidance, eps_out, latents, latents_out, p);
+  if (rc == RTTI_OK) rc = anc_step_args(s_up, z);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale; p.dt_sigma = dt_sigma;
+  p.s_up = s_up; p.z = (const __half*)z;
+  return launch_rescale<false>(p, stream);
+}
+
 extern "C" int rtti_gather_blend_step_rescale(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
                                               const int* slot_owner, int n_slots, int n_regions, const float* masks,
                                               long long n, float guidance, void* eps_out, const void* latents,
@@ -399,5 +440,24 @@ extern "C" int rtti_gather_blend_step_rescale_ms(const void* const* peer_slots, 
   p.phi = guidance_rescale;
   p.ms = MsStep{hx, he, cx, cd, cp, d_prev, d_out};
   p.ms_ref = MsStep{hx, he, cx, cd, cp, d_prev_ref, d_out_ref};
+  return launch_rescale<true>(p, stream);
+}
+
+extern "C" int rtti_gather_blend_step_rescale_anc(const void* const* peer_slots, void* const* peer_flags, int world,
+                                                  int rank, const int* slot_owner, int n_slots, int n_regions,
+                                                  const float* masks, long long n, float guidance, void* eps_out,
+                                                  const void* latents, void* latents_out, const void* latents_ref,
+                                                  void* latents_ref_out, float dt_sigma, float s_up, const void* z,
+                                                  const void* z_ref, unsigned int step_id, float guidance_rescale,
+                                                  void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleAncParams p{};
+  int rc = gather_rescale_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                               eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = anc_step_args(s_up, z);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = anc_step_args(s_up, z_ref);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale; p.dt_sigma = dt_sigma;
+  p.s_up = s_up; p.z = (const __half*)z; p.z_ref = (const __half*)z_ref;
   return launch_rescale<true>(p, stream);
 }

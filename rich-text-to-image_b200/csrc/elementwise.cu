@@ -343,13 +343,14 @@ __global__ void geglu_kernel(const __half* __restrict__ proj, __half* __restrict
 // ============================================================================ region blend + CFG
 struct BlendPtrs { const __half* eps[16]; };
 
-// step policies (rtti_internal.h): Euler, or the multistep update of MsStep
+// step policies (rtti_internal.h): Euler, the multistep update of MsStep, or the ancestral update of AncStep
 struct EulerStep { float dt_sigma; };
 __device__ __forceinline__ void apply_step(const EulerStep& s, long long, const float* e16, float* x) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], s.dt_sigma, x[i]);
 }
 __device__ __forceinline__ void apply_step(const MsStep& s, long long v, const float* e16, float* x) { ms_step8(s, v, e16, x); }
+__device__ __forceinline__ void apply_step(const AncStep& s, long long v, const float* e16, float* x) { anc_step8(s, v, e16, x); }
 
 template <class Step>
 __device__ __forceinline__ void region_blend_body(const __half* __restrict__ eps_uncond, const BlendPtrs& ptrs,
@@ -400,6 +401,13 @@ __global__ void region_blend_ms_kernel(const __half* __restrict__ eps_uncond, Bl
                                        const float* __restrict__ masks, int n_regions, long long n, float guidance,
                                        __half* __restrict__ eps_out, const __half* __restrict__ latents,
                                        __half* __restrict__ latents_out, const MsStep st) {
+  region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
+}
+
+__global__ void region_blend_anc_kernel(const __half* __restrict__ eps_uncond, BlendPtrs ptrs,
+                                        const float* __restrict__ masks, int n_regions, long long n, float guidance,
+                                        __half* __restrict__ eps_out, const __half* __restrict__ latents,
+                                        __half* __restrict__ latents_out, const AncStep st) {
   region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
 }
 
@@ -609,7 +617,7 @@ extern "C" int rtti_geglu_fwd(const void* proj, void* y, int rows, int inner, vo
   return ok_or_cuda();
 }
 
-// argument checks shared by rtti_region_blend_cfg and rtti_region_blend_cfg_ms; fills the region pointer table
+// argument checks shared by rtti_region_blend_cfg and its _ms / _anc forms; fills the region pointer table
 static int region_blend_args(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions,
                              long long n, void* eps_out, const void* latents, void* latents_out, BlendPtrs& ptrs) {
   if (!eps_uncond || !eps_region || !masks || !eps_out) return RTTI_ERR_ARG;
@@ -651,6 +659,21 @@ extern "C" int rtti_region_blend_cfg_ms(const void* eps_uncond, const void* cons
   region_blend_ms_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
       (__half*)latents_out, MsStep{hx, he, cx, cd, cp, d_prev, d_out});
+  return ok_or_cuda();
+}
+
+extern "C" int rtti_region_blend_cfg_anc(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                         int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                         void* latents_out, float dt_sigma, float s_up, const void* z, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  BlendPtrs ptrs{};
+  int rc = region_blend_args(eps_uncond, eps_region, masks, n_regions, n, eps_out, latents, latents_out, ptrs);
+  if (rc == RTTI_OK) rc = anc_step_args(s_up, z);
+  if (rc != RTTI_OK) return rc;
+  const long long nv = n / 8;
+  region_blend_anc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
+      (__half*)latents_out, AncStep{dt_sigma, s_up, (const __half*)z});
   return ok_or_cuda();
 }
 

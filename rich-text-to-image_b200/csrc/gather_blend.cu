@@ -62,13 +62,24 @@ struct GatherBlendMsParams : GatherBlendParams {
   MsStep ms, ms_ref;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep update of the main / reference trajectory
+// the ancestral form: the parameters of the Euler form + the noise of each trajectory
+struct GatherBlendAncParams : GatherBlendParams {
+  float s_up;
+  const __half* z;
+  const __half* z_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral update of the main / reference
+// trajectory
 __device__ __forceinline__ void gb_step(const GatherBlendParams& p, bool, long long, const float* e16, float* x) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
 }
 __device__ __forceinline__ void gb_step(const GatherBlendMsParams& p, bool ref, long long v, const float* e16, float* x) {
   ms_step8(ref ? p.ms_ref : p.ms, v, e16, x);
+}
+__device__ __forceinline__ void gb_step(const GatherBlendAncParams& p, bool ref, long long v, const float* e16, float* x) {
+  anc_step8(AncStep{p.dt_sigma, p.s_up, ref ? p.z_ref : p.z}, v, e16, x);
 }
 
 // steps 1 and 2: publish this rank's step, wait for every peer it reads from. A macro rather than a function: written
@@ -147,6 +158,10 @@ __global__ void __launch_bounds__(128) gather_blend_ms_kernel(const GatherBlendM
   GB_PUBLISH_AND_WAIT(p);
   gather_blend_body(p);
 }
+__global__ void __launch_bounds__(128) gather_blend_anc_kernel(const GatherBlendAncParams p) {
+  GB_PUBLISH_AND_WAIT(p);
+  gather_blend_body(p);
+}
 
 }  // namespace rtti
 
@@ -218,5 +233,28 @@ extern "C" int rtti_gather_blend_step_ms(const void* const* peer_slots, void* co
   p.ms_ref = MsStep{hx, he, cx, cd, cp, d_prev_ref, d_out_ref};
   const long long nv = n / 8;
   gather_blend_ms_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+extern "C" int rtti_gather_blend_step_anc(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                          const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                          long long n, float guidance, void* eps_out, const void* latents,
+                                          void* latents_out, const void* latents_ref, void* latents_ref_out,
+                                          float dt_sigma, float s_up, const void* z, const void* z_ref,
+                                          unsigned int step_id, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  GatherBlendAncParams p{};
+  int rc = gather_blend_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                             eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = anc_step_args(s_up, z);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = anc_step_args(s_up, z_ref);
+  if (rc == RTTI_OK && (((uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out |
+                         (uintptr_t)latents_ref | (uintptr_t)latents_ref_out) & 15))
+    rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.dt_sigma = dt_sigma;
+  p.s_up = s_up; p.z = (const __half*)z; p.z_ref = (const __half*)z_ref;
+  const long long nv = n / 8;
+  gather_blend_anc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

@@ -3,6 +3,9 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#ifdef __CUDACC__
+#include <cuda_fp16.h>
+#endif
 
 #include "../../include/rtti_b200.h"
 
@@ -24,6 +27,12 @@ inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
 inline int ms_step_args(float cp, const float* d_prev, const float* d_out) {
   if (!d_out || (cp != 0.f && !d_prev)) return RTTI_ERR_ARG;
   return (((uintptr_t)d_prev | (uintptr_t)d_out) & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
+}
+
+// the noise of an ancestral blend step: required when s_up != 0, 16-byte aligned
+inline int anc_step_args(float s_up, const void* z) {
+  if (s_up != 0.f && !z) return RTTI_ERR_ARG;
+  return ((uintptr_t)z & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
 }
 
 #ifdef __CUDACC__
@@ -94,6 +103,29 @@ __device__ __forceinline__ void ms_step8(const MsStep& s, long long v, const flo
     float o = fmaf(s.cd, d[i], s.cx * x[i]);
     if (s.cp != 0.f) o = fmaf(s.cp, dp[i], o);
     x[i] = o;
+  }
+}
+
+// The ancestral (Euler a) update: x' = x + dt_sigma * eps + s_up * z, with dt_sigma = sigma_down - sigma and z the
+// fp16 noise of the step, [n] (schedulers.py, EulerAncestralDiscreteScheduler.ancestral_coeffs). The Euler update is
+// formed first, exactly as EulerStep forms it; z is read (128-bit) only when s_up != 0, so s_up = 0 gives the Euler bits.
+struct AncStep {
+  float dt_sigma, s_up;
+  const __half* z;
+};
+
+__device__ __forceinline__ void anc_step8(const AncStep& s, long long v, const float* e16, float* x) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], s.dt_sigma, x[i]);
+  if (s.s_up != 0.f) {
+    const uint4 u = *reinterpret_cast<const uint4*>(s.z + v * 8);
+    const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float2 t = __half22float2(h[i]);
+      x[2 * i] = fmaf(t.x, s.s_up, x[2 * i]);
+      x[2 * i + 1] = fmaf(t.y, s.s_up, x[2 * i + 1]);
+    }
   }
 }
 

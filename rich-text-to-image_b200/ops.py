@@ -246,6 +246,31 @@ class MultistepStep:
         return a + ([_ptr(self.d_prev_ref), _ptr(self.d_out_ref)] if ref else [])
 
 
+class AncestralStep:
+    """The Euler Ancestral update of one blend call: x' = x + dt eps + s_up z, with (dt, s_up) from
+    schedulers.EulerAncestralDiscreteScheduler.ancestral_coeffs and z the fp16 noise of the step, [n] elements (read only
+    when s_up != 0). z_ref: the reference-latent trajectory's noise (gather_blend_step only); both trajectories take the
+    same dt and s_up."""
+
+    def __init__(self, dt, s_up, z, z_ref=None):
+        self.dt, self.s_up = float(dt), float(s_up)
+        self.z, self.z_ref = z, z_ref
+
+    def _check(self, n, ref):
+        for t, name in [(self.z, "z")] + ([(self.z_ref, "z_ref")] if ref else []):
+            if t is None:
+                if self.s_up != 0.0:
+                    raise _lib.RttiError(f"ancestral blend: {name} is required")
+                continue
+            _req(t, _F16, name)
+            if not t.is_contiguous() or t.numel() != n:
+                raise _lib.RttiError(f"ancestral blend: {name} must be a contiguous fp16 tensor of {n} elements")
+
+    def args(self, ref=False):
+        a = [ctypes.c_float(self.dt), ctypes.c_float(self.s_up), _ptr(self.z)]
+        return a + ([_ptr(self.z_ref)] if ref else [])
+
+
 def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0,
                      step=None):
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
@@ -253,7 +278,8 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     guidance_rescale = phi > 0 scales eps by 1 - phi + phi std(eps_t) / std(eps) before it is stored and stepped
     (rtti_region_blend_cfg_rescale); phi == 0 runs rtti_region_blend_cfg.
     step: a MultistepStep — the latents (required then) take the DDIM / DPM-Solver++ update instead of the Euler one
-    (rtti_region_blend_cfg_ms / rtti_region_blend_cfg_rescale_ms; dt_sigma is not used)."""
+    (rtti_region_blend_cfg_ms / rtti_region_blend_cfg_rescale_ms; dt_sigma is not used); an AncestralStep — the
+    Euler Ancestral update (rtti_region_blend_cfg_anc / rtti_region_blend_cfg_rescale_anc; dt_sigma is not used)."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -264,7 +290,20 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    if step is not None:
+    if isinstance(step, AncestralStep):
+        if latents is None:
+            raise _lib.RttiError("region_blend_cfg: an ancestral step needs the latents")
+        step._check(n, False)
+        if guidance_rescale == 0.0:
+            rc = lib.rtti_region_blend_cfg_anc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
+                                               _ptr(latents), _ptr(lat_out), *step.args(), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_anc")
+        else:
+            rc = lib.rtti_region_blend_cfg_rescale_anc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                       _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
+                                                       float(guidance_rescale), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_rescale_anc")
+    elif step is not None:
         if latents is None:
             raise _lib.RttiError("region_blend_cfg: a multistep step needs the latents")
         step._check(n, False)
@@ -358,7 +397,9 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     """Fused all-gather + blend + CFG + Euler over NVLink peer memory (rtti_gather_blend_step; with
     guidance_rescale > 0 rtti_gather_blend_step_rescale, which also rescales the reference-latent pair).
     step: a MultistepStep (with d_prev_ref / d_out_ref when latents_ref is given) — the DDIM / DPM-Solver++ update
-    instead of the Euler one (rtti_gather_blend_step_ms / rtti_gather_blend_step_rescale_ms).
+    instead of the Euler one (rtti_gather_blend_step_ms / rtti_gather_blend_step_rescale_ms); an AncestralStep (with
+    z_ref when latents_ref is given) — the Euler Ancestral update (rtti_gather_blend_step_anc /
+    rtti_gather_blend_step_rescale_anc).
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
@@ -369,7 +410,17 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    if step is not None:
+    if isinstance(step, AncestralStep):
+        step._check(n, latents_ref is not None)
+        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
+                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
+        args += step.args(ref=True) + [int(step_id)]
+        if guidance_rescale == 0.0:
+            _lib.check(lib.rtti_gather_blend_step_anc(*args, _stream()), "rtti_gather_blend_step_anc")
+        else:
+            _lib.check(lib.rtti_gather_blend_step_rescale_anc(*args, float(guidance_rescale), _stream()),
+                       "rtti_gather_blend_step_rescale_anc")
+    elif step is not None:
         step._check(n, latents_ref is not None)
         args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
                 float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]

@@ -9,7 +9,8 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
     reference latent, the input; the hook choreography becomes a RegionControl;
   * region blend + CFG (+ guidance rescale) + scheduler update is one kernel (rtti_region_blend_cfg, or
     rtti_region_blend_cfg_rescale with guidance_rescale > 0; their "_ms" forms for DDIM / DPM-Solver++(2M), which
-    keep one fp32 history of the x0 prediction per trajectory); colour-guidance loss fwd/bwd,
+    keep one fp32 history of the x0 prediction per trajectory, and "_anc" forms for Euler Ancestral, which add the
+    noise drawn for the step); colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
     per-pass noise predictions are all-gathered before the (replicated, deterministic) blend.
@@ -22,7 +23,7 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
-from .schedulers import MULTISTEP_SCHEDULERS, DDIMScheduler, EulerDiscreteScheduler
+from .schedulers import MULTISTEP_SCHEDULERS, DDIMScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -32,15 +33,19 @@ def _rescale_phi(guidance_scale, guidance_rescale):
     return float(guidance_rescale) if guidance_scale > 1.0 and guidance_rescale > 0.0 else 0.0
 
 
-def _is_multistep(scheduler):
-    """False: EulerDiscreteScheduler (the fused Euler update); True: DDIMScheduler / DPMSolverMultistepScheduler (the
-    fused multistep update, step_coeffs). Any other scheduler has no fused update here."""
+def _step_kind(scheduler):
+    """The fused update a scheduler runs as: "euler" (EulerDiscreteScheduler), "ancestral"
+    (EulerAncestralDiscreteScheduler: the Euler update plus the noise term, ancestral_coeffs) or "multistep"
+    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs). Any other scheduler has no fused update here."""
+    if isinstance(scheduler, EulerAncestralDiscreteScheduler):
+        return "ancestral"
     if isinstance(scheduler, EulerDiscreteScheduler):
-        return False
+        return "euler"
     if isinstance(scheduler, MULTISTEP_SCHEDULERS):
-        return True
+        return "multistep"
     raise TypeError(f"RegionDiffusionXL: unsupported scheduler {type(scheduler).__name__}; supported: "
-                    "EulerDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler (rtti_b200.schedulers)")
+                    "EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler "
+                    "(rtti_b200.schedulers)")
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -210,8 +215,18 @@ class RegionDiffusionXL:
         With a multistep scheduler the rich-text pass keeps one history per trajectory: where the reference steps the
         reference latents jointly with the main latents only on a prefix of the steps (inject_selfattn = 0,
         0 < inject_background < 1, :831-846) and then steps the main latents alone, the main latents keep their own
-        history here instead of continuing a batch-2 one."""
-        multistep = _is_multistep(self.scheduler)
+        history here instead of continuing a batch-2 one.
+        With EulerAncestralDiscreteScheduler the noise z of each step is drawn as diffusers' randn_tensor draws it, fp16,
+        from `generator` when one is given (on its device: a CPU generator draws on the CPU), otherwise from the global
+        RNG of the sampling device. The plain pass draws [1, ...] per step, as the reference does. The rich-text pass
+        draws one [2, ...] tensor on the steps where the reference steps the main and reference latents jointly (first
+        half to the main latents, second half to the reference latents) and [1, ...] on the others. Unlike the reference,
+        which passes no generator to the rich-text pass's step, that pass also draws from `generator`: a seeded run is
+        reproducible from start to end. With generator=None both passes draw exactly what the reference draws. On more
+        than one GPU every rank must add the same noise: sample() compares a digest of the noise source's state over
+        the ranks once and raises on every rank if they disagree."""
+        kind = _step_kind(self.scheduler)
+        multistep = kind == "multistep"
         if multistep and eta > 0 and not run_rich_text and isinstance(self.scheduler, DDIMScheduler):
             raise NotImplementedError("RegionDiffusionXL: DDIM with eta > 0 is not implemented")
         height = height or self.default_sample_size * self.vae_scale_factor
@@ -227,6 +242,8 @@ class RegionDiffusionXL:
         pooled = torch.cat([negative_pooled_prompt_embeds, pooled_prompt_embeds], 0).to(dev, torch.float16)
         time_ids = torch.tensor([list(original_size) + list(crops_coords_top_left) + list(target_size)],
                                 dtype=torch.float32, device=dev)
+        if kind == "ancestral":
+            region_parallel.check_noise_source(generator, dev, group=self.region_group)
         self.scheduler.set_timesteps(num_inference_steps, device=dev)
         timesteps = self.scheduler.timesteps
         latents = self.prepare_latents(height, width, generator, latents)
@@ -234,10 +251,10 @@ class RegionDiffusionXL:
         if run_rich_text:
             latents = self._rich_text_loop(ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
                                            inject_selfattn, inject_background, text_format_dict or {}, callback,
-                                           callback_steps, guidance_rescale)
+                                           callback_steps, guidance_rescale, generator)
         else:
             latents = self._plain_loop(ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps,
-                                       guidance_rescale)
+                                       guidance_rescale, generator)
 
         if output_type == "latent":
             return StableDiffusionXLPipelineOutput(images=latents)
@@ -252,16 +269,19 @@ class RegionDiffusionXL:
         return StableDiffusionXLPipelineOutput(images=[Image.fromarray(a) for a in arr])
 
     def _plain_loop(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps,
-                    guidance_rescale=0.0):
+                    guidance_rescale=0.0, generator=None):
         """:879-914 — CFG batch [uncond, cond]; with capture armed the attention kernels accumulate the maps.
         guidance_rescale rescales the CFG prediction inside the blend kernel (:903-905). A multistep scheduler: the UNet
-        sees the latents unscaled and the blend kernel takes the step_coeffs(i) update."""
+        sees the latents unscaled and the blend kernel takes the step_coeffs(i) update. Euler Ancestral: the UNet input
+        is scaled as for Euler and the blend kernel adds s_up z, z [1, ...] drawn from `generator` after the UNet pass,
+        as the reference's step draws it (:908)."""
         phi = _rescale_phi(guidance_scale, guidance_rescale)
         ctx2 = torch.cat([ctx[:1], ctx[-1:]])
         pooled2 = torch.cat([pooled[:1], pooled[-1:]])
         kv = CrossKVCache()
         ones = None
-        multistep = _is_multistep(self.scheduler)
+        kind = _step_kind(self.scheduler)
+        multistep = kind == "multistep"
         d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=latents.device) if multistep else None
         for i, t in enumerate(timesteps):
             if multistep:
@@ -278,6 +298,12 @@ class RegionDiffusionXL:
                 step = ops.MultistepStep(self.scheduler.step_coeffs(i), d_hist, d_hist)
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(), guidance_rescale=phi, step=step)
+            elif kind == "ancestral":
+                dt, s_up = self.scheduler.ancestral_coeffs(i)
+                z = self.scheduler.noise(tuple(latents.shape), generator, latents.device)
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=latents.contiguous(), guidance_rescale=phi,
+                                                  step=ops.AncestralStep(dt, s_up, z))
             else:
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
@@ -298,10 +324,11 @@ class RegionDiffusionXL:
         return passes
 
     def prepare_rich_text(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
-                          inject_selfattn, inject_background, tfd, guidance_rescale=0.0):
+                          inject_selfattn, inject_background, tfd, guidance_rescale=0.0, generator=None):
         """Everything of :772-778 that is constant over the steps, as a state object for rich_text_step().
         guidance_rescale: the CFG rescale the reference leaves as a TODO (:827-830), applied to the blended prediction
-        (eps_text = the masked sum of the text passes) and, when it is stepped, to the reference-latent pair C/D."""
+        (eps_text = the masked sum of the text passes) and, when it is stepped, to the reference-latent pair C/D.
+        generator: the source of Euler Ancestral's noise (None: the global RNG of the sampling device)."""
         dev = self.device
         N = len(self.masks)
         assert ctx.shape[0] == N + 1, "prompts must be [region_1..region_{N-1}, base] matching self.masks"
@@ -334,7 +361,9 @@ class RegionDiffusionXL:
         st.graphs = {}
         st.noise_pred = None
         # multistep schedulers: one fp32 history of the x0 prediction per trajectory (main, reference)
-        st.multistep = _is_multistep(self.scheduler)
+        kind = _step_kind(self.scheduler)
+        st.multistep, st.ancestral = kind == "multistep", kind == "ancestral"
+        st.generator = generator
         n = latents.numel()
         st.d_hist = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep else None
         st.d_hist_ref = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep and inject else None
@@ -457,14 +486,25 @@ class RegionDiffusionXL:
                 rq.end_pass()
         if pe is not None:
             ev[1].record()
+        step_ref = st.inject and (st.inject_selfattn > 0 or background_inject_step)                       # :830-841
         if st.multistep:
             c = self.scheduler.step_coeffs(i)
             dt = 0.0
             step = ops.MultistepStep(c, st.d_hist, st.d_hist, st.d_hist_ref, st.d_hist_ref)
+            step_main = ops.MultistepStep(c, st.d_hist, st.d_hist)
+            step_refl = ops.MultistepStep(c, st.d_hist_ref, st.d_hist_ref)
+        elif st.ancestral:
+            # the reference draws z in its scheduler step (:837-846): one [2, ...] draw when it steps both trajectories
+            # as one batch (main first), [1, ...] otherwise; on CUDA one [2, n] draw differs from two [1, n] draws
+            dt = 0.0
+            a_dt, s_up = self.scheduler.ancestral_coeffs(i)
+            z = self.scheduler.noise((2 if step_ref else 1,) + tuple(st.latents.shape[1:]), st.generator, self.device)
+            z_ref = z[1:2] if step_ref else None
+            step = ops.AncestralStep(a_dt, s_up, z[0:1], z_ref)
+            step_main, step_refl = ops.AncestralStep(a_dt, s_up, z[0:1]), ops.AncestralStep(a_dt, s_up, z_ref)
         else:
             dt = self.scheduler.dt(t)
-            step = None
-        step_ref = st.inject and (st.inject_selfattn > 0 or background_inject_step)                       # :830-841
+            step = step_main = step_refl = None
         ex = None
         if plan.world > 1 and self.fused_exchange:
             xkey = (tuple(p["kind"] for p in passes), st.latents[0].numel())
@@ -477,7 +517,7 @@ class RegionDiffusionXL:
                     self.fused_exchange = False
             ex = self._exchanges.get(xkey)
         if ex is not None:
-            # fused all-gather + blend + CFG + Euler over NVLink peer memory (csrc/gather_blend.cu)
+            # fused all-gather + blend + CFG + scheduler update over NVLink peer memory (csrc/gather_blend.cu)
             _, owner = plan._plan(feat_inject_step)
             sid = ex.publish(eps_local, local, owner)
             st.noise_pred, st.latents, ref_out = ops.gather_blend_step(
@@ -493,12 +533,12 @@ class RegionDiffusionXL:
             st.noise_pred, st.latents = ops.region_blend_cfg(one("A"), regions, st.masks, st.guidance_scale,
                                                               latents=st.latents.contiguous(), dt_sigma=dt,
                                                               guidance_rescale=st.guidance_rescale,
-                                                              step=ops.MultistepStep(c, st.d_hist, st.d_hist) if step else None)  # :810-830
+                                                              step=step_main)  # :810-830
             if step_ref:
                 _, st.latents_ref = ops.region_blend_cfg(one("C"), [one("D")], st.ones, st.guidance_scale,
                                                          latents=st.latents_ref.contiguous(), dt_sigma=dt,
                                                          guidance_rescale=st.guidance_rescale,
-                                                         step=ops.MultistepStep(c, st.d_hist_ref, st.d_hist_ref) if step else None)
+                                                         step=step_refl)
         if pe is not None:
             ev[2].record()
         if st.use_guidance and float(t) < st.tfd["guidance_start_step"]:                                  # :849
@@ -513,10 +553,11 @@ class RegionDiffusionXL:
         return st.latents
 
     def _rich_text_loop(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
-                        inject_selfattn, inject_background, tfd, callback, callback_steps, guidance_rescale=0.0):
+                        inject_selfattn, inject_background, tfd, callback, callback_steps, guidance_rescale=0.0,
+                        generator=None):
         """:772-878."""
         st = self.prepare_rich_text(ctx, pooled, time_ids, latents, timesteps, guidance_scale, use_guidance,
-                                    inject_selfattn, inject_background, tfd, guidance_rescale)
+                                    inject_selfattn, inject_background, tfd, guidance_rescale, generator)
         for i, t in enumerate(timesteps):
             self.rich_text_step(st, i)
             if callback is not None and i % callback_steps == 0:

@@ -15,6 +15,7 @@ pass D (:1018-1061). So:
     the blend + CFG + scheduler update is replicated on every rank — it is deterministic, so the
     latents stay bit-identical across ranks without a broadcast.
 """
+import hashlib
 from typing import List
 
 import torch
@@ -25,6 +26,37 @@ def _dist():
     if dist.is_available() and dist.is_initialized():
         return dist
     return None
+
+
+def noise_source_digest(generator=None, device=None):
+    """64-bit digest of the state a stochastic sampler draws its noise from: `generator`, or the global RNG of `device`
+    (torch.cuda's for a CUDA device, torch's CPU RNG otherwise)."""
+    if generator is not None:
+        state = generator.get_state()
+    elif device is not None and torch.device(device).type == "cuda":
+        state = torch.cuda.get_rng_state(device)
+    else:
+        state = torch.get_rng_state()
+    return int.from_bytes(hashlib.blake2b(state.numpy().tobytes(), digest_size=8).digest(), "little", signed=True)
+
+
+def check_noise_source(generator=None, device=None, group=None):
+    """Collective over `group` (None: all ranks) when more than one rank takes part: raise on every rank unless all ranks
+    hold the same noise-source state (noise_source_digest). The blends are replicated on every rank, so ranks that add
+    different noise would drift apart without any other error."""
+    dist = _dist()
+    if dist is None or dist.get_world_size(group) <= 1:
+        return
+    backend = dist.get_backend(group)
+    dev = torch.device(device) if backend == "nccl" else torch.device("cpu")
+    mine = torch.tensor([noise_source_digest(generator, device)], dtype=torch.int64, device=dev)
+    every = [torch.empty_like(mine) for _ in range(dist.get_world_size(group))]
+    dist.all_gather(every, mine, group=group)
+    digests = [int(d) for d in every]
+    if len(set(digests)) > 1:
+        what = "generator" if generator is not None else "global RNG of the sampling device"
+        raise RuntimeError(f"rtti_b200: the ranks' noise sources differ (the {what}; digests by rank "
+                           f"{[f'{d & (2 ** 64 - 1):016x}' for d in digests]}): seed it identically on every rank")
 
 
 def assign_passes_balanced(kinds: List[str], world: int):

@@ -8,7 +8,8 @@ init_noise_sigma / alphas_cumprod.  All state lives on the sampling device; `ste
 
 DDIMScheduler and DPMSolverMultistepScheduler (below) are the schedulers a diffusers user swaps in
 (`model.scheduler = DPMSolverMultistepScheduler(...)`); the samplers run them through the fused blend kernels with
-the per-step coefficients of `step_coeffs(i)`.
+the per-step coefficients of `step_coeffs(i)`. EulerAncestralDiscreteScheduler ("Euler a", SDXL) adds fresh noise on
+every step; the SDXL sampler runs it through the fused blend kernels with `ancestral_coeffs(i)`.
 """
 import math
 from typing import NamedTuple
@@ -144,17 +145,12 @@ class StepCoeffs(NamedTuple):
     cp: float
 
 
-class _MultistepBase:
-    """Shared VP-space conventions of DDIMScheduler and DPMSolverMultistepScheduler: scaled-linear betas, epsilon
-    prediction, init_noise_sigma = 1, scale_model_input = identity (the UNet sees the latents unscaled),
-    alphas_cumprod = the same host fp32 tensor as the other schedulers (colour guidance's predict_x0), host int64
-    timesteps. Write a_t = alphas_cumprod[t], alpha_t = sqrt(a_t), sigma_t = sqrt(1 - a_t),
-    lambda_t = log alpha_t - log sigma_t."""
-    order = 1
-    init_noise_sigma = 1.0
-    _unsupported = {}  # keyword -> the only value this restatement implements
+class _Configured:
+    """Keyword configuration of the schedulers a diffusers user swaps in: `_defaults` (diffusers' keywords and defaults)
+    and `_unsupported` (keyword -> the only value this restatement implements)."""
+    _unsupported = {}
 
-    def __init__(self, **kw):
+    def _configure(self, kw):
         for k, v in kw.items():
             if k in self._unsupported and v != self._unsupported[k]:
                 raise NotImplementedError(f"{type(self).__name__}: {k}={v!r} is not supported "
@@ -167,14 +163,7 @@ class _MultistepBase:
         if cfg["beta_schedule"] != "scaled_linear":
             raise NotImplementedError(f"{type(self).__name__}: beta_schedule={cfg['beta_schedule']!r} is not supported")
         self.config = _Config(cfg)
-        self.num_train_timesteps = int(cfg["num_train_timesteps"])
-        self.alphas_cumprod = _alphas_cumprod(cfg["beta_start"], cfg["beta_end"], self.num_train_timesteps)
-        ac = self.alphas_cumprod.double().numpy()
-        self._alpha, self._sigma = np.sqrt(ac), np.sqrt(1.0 - ac)
-        self._lambda = np.log(self._alpha) - np.log(self._sigma)
-        self.timesteps = None
-        self.num_inference_steps = None
-        self._d_prev = None
+        return self.config
 
     @classmethod
     def from_config(cls, config, **kw):
@@ -183,6 +172,27 @@ class _MultistepBase:
         cfg = dict(config if isinstance(config, dict) else config.config)
         cfg.update(kw)
         return cls(**{k: v for k, v in cfg.items() if k in cls._defaults})
+
+
+class _MultistepBase(_Configured):
+    """Shared VP-space conventions of DDIMScheduler and DPMSolverMultistepScheduler: scaled-linear betas, epsilon
+    prediction, init_noise_sigma = 1, scale_model_input = identity (the UNet sees the latents unscaled),
+    alphas_cumprod = the same host fp32 tensor as the other schedulers (colour guidance's predict_x0), host int64
+    timesteps. Write a_t = alphas_cumprod[t], alpha_t = sqrt(a_t), sigma_t = sqrt(1 - a_t),
+    lambda_t = log alpha_t - log sigma_t."""
+    order = 1
+    init_noise_sigma = 1.0
+
+    def __init__(self, **kw):
+        cfg = self._configure(kw)
+        self.num_train_timesteps = int(cfg["num_train_timesteps"])
+        self.alphas_cumprod = _alphas_cumprod(cfg["beta_start"], cfg["beta_end"], self.num_train_timesteps)
+        ac = self.alphas_cumprod.double().numpy()
+        self._alpha, self._sigma = np.sqrt(ac), np.sqrt(1.0 - ac)
+        self._lambda = np.log(self._alpha) - np.log(self._sigma)
+        self.timesteps = None
+        self.num_inference_steps = None
+        self._d_prev = None
 
     def scale_model_input(self, sample, timestep=None):
         return sample
@@ -280,3 +290,76 @@ class DPMSolverMultistepScheduler(_MultistepBase):
 
 
 MULTISTEP_SCHEDULERS = (DDIMScheduler, DPMSolverMultistepScheduler)
+
+
+# ---------------------------------------------------------------------------------------------------- ancestral
+class EulerAncestralDiscreteScheduler(_Configured):
+    """Euler Ancestral ("Euler a"), epsilon prediction, with the SDXL config (scaled-linear betas 0.00085-0.012, `leading`
+    spacing, steps_offset=1), restating diffusers 0.18.2 (`schedulers/scheduling_euler_ancestral_discrete.py`). PARITY
+    UNPINNED: that source is not available here; the conventions below are the definition.
+      timesteps, sigmas_host, init_noise_sigma, scale_model_input, alphas_cumprod: those of EulerDiscreteScheduler
+      step i, sigma = sigmas_host[i] -> sigma' = sigmas_host[i + 1]:
+        s_up = sqrt(sigma'^2 (sigma^2 - sigma'^2) / sigma^2),  s_down = sqrt(sigma'^2 - s_up^2)
+        x' = x + (s_down - sigma) eps + s_up z
+      z ~ N(0, 1), drawn as diffusers' randn_tensor draws it (`noise`), on every step: also on the last one, where
+      sigma' = 0 and so s_up = 0.
+    Not a subclass of EulerDiscreteScheduler: its `dt` is not this scheduler's step. The samplers run it through the
+    fused blend kernels with the coefficients of `ancestral_coeffs(i)`."""
+    order = 1
+    _defaults = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                     trained_betas=None, prediction_type="epsilon", timestep_spacing="leading", steps_offset=1)
+    _unsupported = dict(trained_betas=None, prediction_type="epsilon", timestep_spacing="leading")
+
+    def __init__(self, **kw):
+        cfg = self._configure(kw)
+        self._grid = EulerDiscreteScheduler(cfg["beta_start"], cfg["beta_end"], int(cfg["num_train_timesteps"]),
+                                            int(cfg["steps_offset"]))
+        self.num_train_timesteps = self._grid.num_train_timesteps
+        self.alphas_cumprod = self._grid.alphas_cumprod
+        self.num_inference_steps = None
+        self._take_grid()
+
+    def _take_grid(self):
+        self.timesteps, self.timesteps_host, self.sigmas_host = \
+            self._grid.timesteps, self._grid.timesteps_host, self._grid.sigmas_host
+
+    @property
+    def init_noise_sigma(self):
+        return self._grid.init_noise_sigma
+
+    def set_timesteps(self, num_inference_steps, device=None):
+        self._grid.set_timesteps(num_inference_steps, device)
+        self.num_inference_steps = num_inference_steps
+        self._take_grid()
+
+    def index_of(self, timestep):
+        return self._grid.index_of(timestep)
+
+    def sigma(self, timestep):
+        return self._grid.sigma(timestep)
+
+    def scale_model_input(self, sample, timestep):
+        return self._grid.scale_model_input(sample, timestep)
+
+    def ancestral_coeffs(self, i):
+        """(dt, s_up) of step i in float64: x' = x + dt eps + s_up z, dt = s_down - sigma."""
+        s, s_to = float(self.sigmas_host[i]), float(self.sigmas_host[i + 1])
+        s_up = math.sqrt(s_to * s_to * (s * s - s_to * s_to) / (s * s))
+        s_down = math.sqrt(s_to * s_to - s_up * s_up)
+        return s_down - s, s_up
+
+    @staticmethod
+    def noise(shape, generator=None, device=None, dtype=torch.float16):
+        """z of one step as diffusers' randn_tensor draws it: from `generator` on the generator's device (a CPU generator
+        draws on the CPU and the result is copied to `device`), or, without one, from the global RNG of `device`."""
+        if generator is None:
+            return torch.randn(shape, dtype=dtype, device=device)
+        return torch.randn(shape, dtype=dtype, generator=generator, device=generator.device).to(device)
+
+    def step(self, model_output, timestep, sample, generator=None, return_dict=True, **kw):
+        """Torch form of ancestral_coeffs (the samplers use the fused kernels instead); z has model_output's shape and
+        dtype."""
+        dt, s_up = self.ancestral_coeffs(self.index_of(timestep))
+        z = self.noise(model_output.shape, generator, model_output.device, model_output.dtype)
+        prev = (sample.float() + model_output.float() * dt + z.float() * s_up).to(sample.dtype)
+        return {"prev_sample": prev} if return_dict else (prev,)
