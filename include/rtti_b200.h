@@ -173,6 +173,30 @@ int rtti_region_blend_cfg_rescale_anc(const void* eps_uncond, const void* const*
                                       void* latents_out, float dt_sigma, float s_up, const void* z,
                                       float guidance_rescale, void* stream);
 
+/* UniPC forms ("_unipc") of the blend entry points, for UniPC bh2 of order 2 (rich-text-to-image_b200/schedulers.py,
+ * UniPCMultistepScheduler.unipc_coeffs). The blend, CFG and rescale arithmetic is that of the Euler form; the update of
+ * the latents is, in fp32,
+ *   m  = hx * x + he * eps                                   (written to m_out[n])
+ *   xc = ux * x + ul * xl + u0 * m + u1 * m1 + u2 * m2       (the corrected sample, written to xl_out[n])
+ *   x' = vx * xc + v0 * m + v1 * m1                          (x' rounded to fp16)
+ * with x the fp16 latents, eps the fp16-rounded noise prediction written to eps_out, and xl, m1, m2 the fp32 [n]
+ * histories (xc of the previous step, m of the previous two steps). latents, latents_out, m_out and xl_out are required;
+ * xl may be null only when ul == 0, m1 only when u1 == v1 == 0, m2 only when u2 == 0, and a history is read only when
+ * one of its coefficients is non-zero. m_out may alias m2 and xl_out may alias xl (every element is read before it is
+ * written, by the same thread). Histories 16-byte aligned. The other checks are those of the Euler form; on any error
+ * nothing is launched. */
+int rtti_region_blend_cfg_unipc(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                void* latents_out, float hx, float he, float ux, float ul, float u0, float u1,
+                                float u2, float vx, float v0, float v1, const float* xl, const float* m1,
+                                const float* m2, float* m_out, float* xl_out, void* stream);
+int rtti_region_blend_cfg_rescale_unipc(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                        int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                        void* latents_out, float hx, float he, float ux, float ul, float u0, float u1,
+                                        float u2, float vx, float v0, float v1, const float* xl, const float* m1,
+                                        const float* m2, float* m_out, float* xl_out, float guidance_rescale,
+                                        void* stream);
+
 /* Colour-guidance loss forward + analytic backward w.r.t. the VAE decoder output.
  * Replaces models/region_diffusion_sdxl.py:857-865 (clamp, masked mean RGB, MSE*100, autograd of those).
  *   decoded [3, hw] fp32 (VAE output before /2+0.5), masks [n_colors, hw] fp32 (channel 0 of
@@ -290,6 +314,29 @@ int rtti_gather_blend_step_rescale_anc(const void* const* peer_slots, void* cons
                                        void* latents_out, const void* latents_ref, void* latents_ref_out,
                                        float dt_sigma, float s_up, const void* z, const void* z_ref,
                                        unsigned int step_id, float guidance_rescale, void* stream);
+
+/* UniPC forms of rtti_gather_blend_step / rtti_gather_blend_step_rescale (the update of rtti_region_blend_cfg_unipc).
+ * The reference-latent trajectory, when latents_ref is given, is stepped with the same coefficients on its own three
+ * histories (xl_ref, m1_ref, m2_ref -> m_out_ref, xl_out_ref, with the requirements of the main ones). For the same
+ * noise predictions the outputs equal those of the single-GPU forms (the C/D pair: one region and a mask of ones) bit
+ * for bit, whatever the world size. Same protocol and slot layout as the Euler forms. */
+int rtti_gather_blend_step_unipc(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                 const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                                 float guidance, void* eps_out, const void* latents, void* latents_out,
+                                 const void* latents_ref, void* latents_ref_out, float hx, float he, float ux, float ul,
+                                 float u0, float u1, float u2, float vx, float v0, float v1, const float* xl,
+                                 const float* m1, const float* m2, float* m_out, float* xl_out, const float* xl_ref,
+                                 const float* m1_ref, const float* m2_ref, float* m_out_ref, float* xl_out_ref,
+                                 unsigned int step_id, void* stream);
+int rtti_gather_blend_step_rescale_unipc(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                         const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                         long long n, float guidance, void* eps_out, const void* latents,
+                                         void* latents_out, const void* latents_ref, void* latents_ref_out, float hx,
+                                         float he, float ux, float ul, float u0, float u1, float u2, float vx,
+                                         float v0, float v1, const float* xl, const float* m1, const float* m2,
+                                         float* m_out, float* xl_out, const float* xl_ref, const float* m1_ref,
+                                         const float* m2_ref, float* m_out_ref, float* xl_out_ref,
+                                         unsigned int step_id, float guidance_rescale, void* stream);
 
 /* Stripe-parallel colour guidance (multi-GPU; new relative to the single-GPU reference, which back-propagates
  * through the batch-1 VAE decoder on one device: models/region_diffusion_sdxl.py:849-867). Every activation of

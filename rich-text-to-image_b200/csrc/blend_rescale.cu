@@ -66,8 +66,13 @@ struct RescaleAncParams : RescaleParams {
   const __half* z_ref;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral update of the main (REF false) /
-// reference (REF true) trajectory
+// the UniPC form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory
+struct RescaleUniPCParams : RescaleParams {
+  UniPCStep up, up_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC update of the main (REF
+// false) / reference (REF true) trajectory
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleParams& p, long long, const float* e16, float* x) {
 #pragma unroll
@@ -80,6 +85,10 @@ __device__ __forceinline__ void rs_step(const RescaleMsParams& p, long long v, c
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleAncParams& p, long long v, const float* e16, float* x) {
   anc_step8(AncStep{p.dt_sigma, p.s_up, REF ? p.z_ref : p.z}, v, e16, x);
+}
+template <bool REF>
+__device__ __forceinline__ void rs_step(const RescaleUniPCParams& p, long long v, const float* e16, float* x) {
+  unipc_step8(REF ? p.up_ref : p.up, v, e16, x);
 }
 
 // (count, mean, m2) of eps_text and of eps_cfg over the same elements
@@ -276,6 +285,14 @@ __global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
   blend_rescale_body<PEER>(p, cfg_s, sm);
 }
 
+template <bool PEER>
+__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
+    blend_rescale_unipc_kernel(const __grid_constant__ RescaleUniPCParams p) {
+  extern __shared__ float4 cfg_s[];
+  __shared__ RescaleSmem sm;
+  blend_rescale_body<PEER>(p, cfg_s, sm);
+}
+
 // the kernel of each parameter type
 template <bool PEER>
 const void* rescale_kernel(const RescaleParams&) { return (const void*)blend_rescale_kernel<PEER>; }
@@ -283,6 +300,8 @@ template <bool PEER>
 const void* rescale_kernel(const RescaleMsParams&) { return (const void*)blend_rescale_ms_kernel<PEER>; }
 template <bool PEER>
 const void* rescale_kernel(const RescaleAncParams&) { return (const void*)blend_rescale_anc_kernel<PEER>; }
+template <bool PEER>
+const void* rescale_kernel(const RescaleUniPCParams&) { return (const void*)blend_rescale_unipc_kernel<PEER>; }
 
 // threads per CTA and vectors per thread: a function of n only
 void rescale_plan(long long n, int& threads, int& vpt) {
@@ -306,6 +325,8 @@ int launch_rescale(P& p, void* stream) {
     blend_rescale_ms_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else if constexpr (std::is_same<P, RescaleAncParams>::value)
     blend_rescale_anc_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
+  else if constexpr (std::is_same<P, RescaleUniPCParams>::value)
+    blend_rescale_unipc_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else
     blend_rescale_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
@@ -459,5 +480,46 @@ extern "C" int rtti_gather_blend_step_rescale_anc(const void* const* peer_slots,
   if (rc != RTTI_OK) return rc;
   p.phi = guidance_rescale; p.dt_sigma = dt_sigma;
   p.s_up = s_up; p.z = (const __half*)z; p.z_ref = (const __half*)z_ref;
+  return launch_rescale<true>(p, stream);
+}
+
+extern "C" int rtti_region_blend_cfg_rescale_unipc(const void* eps_uncond, const void* const* eps_region,
+                                                   const float* masks, int n_regions, long long n, float guidance,
+                                                   void* eps_out, const void* latents, void* latents_out, float hx,
+                                                   float he, float ux, float ul, float u0, float u1, float u2,
+                                                   float vx, float v0, float v1, const float* xl, const float* m1,
+                                                   const float* m2, float* m_out, float* xl_out,
+                                                   float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleUniPCParams p{};
+  int rc = rescale_args(eps_uncond, eps_region, masks, n_regions, n, guidance, eps_out, latents, latents_out, p);
+  if (rc == RTTI_OK) rc = unipc_step_args(ul, u1, u2, v1, xl, m1, m2, m_out, xl_out);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.up = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl, m1, m2, m_out, xl_out};
+  return launch_rescale<false>(p, stream);
+}
+
+extern "C" int rtti_gather_blend_step_rescale_unipc(const void* const* peer_slots, void* const* peer_flags, int world,
+                                                    int rank, const int* slot_owner, int n_slots, int n_regions,
+                                                    const float* masks, long long n, float guidance, void* eps_out,
+                                                    const void* latents, void* latents_out, const void* latents_ref,
+                                                    void* latents_ref_out, float hx, float he, float ux, float ul,
+                                                    float u0, float u1, float u2, float vx, float v0, float v1,
+                                                    const float* xl, const float* m1, const float* m2, float* m_out,
+                                                    float* xl_out, const float* xl_ref, const float* m1_ref,
+                                                    const float* m2_ref, float* m_out_ref, float* xl_out_ref,
+                                                    unsigned int step_id, float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleUniPCParams p{};
+  int rc = gather_rescale_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                               eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = unipc_step_args(ul, u1, u2, v1, xl, m1, m2, m_out, xl_out);
+  if (rc == RTTI_OK && latents_ref != nullptr)
+    rc = unipc_step_args(ul, u1, u2, v1, xl_ref, m1_ref, m2_ref, m_out_ref, xl_out_ref);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.up = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl, m1, m2, m_out, xl_out};
+  p.up_ref = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl_ref, m1_ref, m2_ref, m_out_ref, xl_out_ref};
   return launch_rescale<true>(p, stream);
 }

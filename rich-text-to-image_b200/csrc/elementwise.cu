@@ -343,7 +343,8 @@ __global__ void geglu_kernel(const __half* __restrict__ proj, __half* __restrict
 // ============================================================================ region blend + CFG
 struct BlendPtrs { const __half* eps[16]; };
 
-// step policies (rtti_internal.h): Euler, the multistep update of MsStep, or the ancestral update of AncStep
+// step policies (rtti_internal.h): Euler, the multistep update of MsStep, the ancestral update of AncStep, or the UniPC
+// update of UniPCStep
 struct EulerStep { float dt_sigma; };
 __device__ __forceinline__ void apply_step(const EulerStep& s, long long, const float* e16, float* x) {
 #pragma unroll
@@ -351,6 +352,9 @@ __device__ __forceinline__ void apply_step(const EulerStep& s, long long, const 
 }
 __device__ __forceinline__ void apply_step(const MsStep& s, long long v, const float* e16, float* x) { ms_step8(s, v, e16, x); }
 __device__ __forceinline__ void apply_step(const AncStep& s, long long v, const float* e16, float* x) { anc_step8(s, v, e16, x); }
+__device__ __forceinline__ void apply_step(const UniPCStep& s, long long v, const float* e16, float* x) {
+  unipc_step8(s, v, e16, x);
+}
 
 template <class Step>
 __device__ __forceinline__ void region_blend_body(const __half* __restrict__ eps_uncond, const BlendPtrs& ptrs,
@@ -408,6 +412,13 @@ __global__ void region_blend_anc_kernel(const __half* __restrict__ eps_uncond, B
                                         const float* __restrict__ masks, int n_regions, long long n, float guidance,
                                         __half* __restrict__ eps_out, const __half* __restrict__ latents,
                                         __half* __restrict__ latents_out, const AncStep st) {
+  region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
+}
+
+__global__ void region_blend_unipc_kernel(const __half* __restrict__ eps_uncond, BlendPtrs ptrs,
+                                          const float* __restrict__ masks, int n_regions, long long n, float guidance,
+                                          __half* __restrict__ eps_out, const __half* __restrict__ latents,
+                                          __half* __restrict__ latents_out, const UniPCStep st) {
   region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
 }
 
@@ -617,7 +628,7 @@ extern "C" int rtti_geglu_fwd(const void* proj, void* y, int rows, int inner, vo
   return ok_or_cuda();
 }
 
-// argument checks shared by rtti_region_blend_cfg and its _ms / _anc forms; fills the region pointer table
+// argument checks shared by rtti_region_blend_cfg and its _ms / _anc / _unipc forms; fills the region pointer table
 static int region_blend_args(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions,
                              long long n, void* eps_out, const void* latents, void* latents_out, BlendPtrs& ptrs) {
   if (!eps_uncond || !eps_region || !masks || !eps_out) return RTTI_ERR_ARG;
@@ -674,6 +685,24 @@ extern "C" int rtti_region_blend_cfg_anc(const void* eps_uncond, const void* con
   region_blend_anc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
       (__half*)latents_out, AncStep{dt_sigma, s_up, (const __half*)z});
+  return ok_or_cuda();
+}
+
+extern "C" int rtti_region_blend_cfg_unipc(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                           int n_regions, long long n, float guidance, void* eps_out,
+                                           const void* latents, void* latents_out, float hx, float he, float ux,
+                                           float ul, float u0, float u1, float u2, float vx, float v0, float v1,
+                                           const float* xl, const float* m1, const float* m2, float* m_out,
+                                           float* xl_out, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  BlendPtrs ptrs{};
+  int rc = region_blend_args(eps_uncond, eps_region, masks, n_regions, n, eps_out, latents, latents_out, ptrs);
+  if (rc == RTTI_OK) rc = unipc_step_args(ul, u1, u2, v1, xl, m1, m2, m_out, xl_out);
+  if (rc != RTTI_OK) return rc;
+  const long long nv = n / 8;
+  region_blend_unipc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
+      (__half*)latents_out, UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl, m1, m2, m_out, xl_out});
   return ok_or_cuda();
 }
 

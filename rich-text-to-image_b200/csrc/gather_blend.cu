@@ -69,8 +69,13 @@ struct GatherBlendAncParams : GatherBlendParams {
   const __half* z_ref;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral update of the main / reference
-// trajectory
+// the UniPC form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory
+struct GatherBlendUniPCParams : GatherBlendParams {
+  UniPCStep up, up_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC update of the main /
+// reference trajectory
 __device__ __forceinline__ void gb_step(const GatherBlendParams& p, bool, long long, const float* e16, float* x) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
@@ -80,6 +85,10 @@ __device__ __forceinline__ void gb_step(const GatherBlendMsParams& p, bool ref, 
 }
 __device__ __forceinline__ void gb_step(const GatherBlendAncParams& p, bool ref, long long v, const float* e16, float* x) {
   anc_step8(AncStep{p.dt_sigma, p.s_up, ref ? p.z_ref : p.z}, v, e16, x);
+}
+__device__ __forceinline__ void gb_step(const GatherBlendUniPCParams& p, bool ref, long long v, const float* e16,
+                                        float* x) {
+  unipc_step8(ref ? p.up_ref : p.up, v, e16, x);
 }
 
 // steps 1 and 2: publish this rank's step, wait for every peer it reads from. A macro rather than a function: written
@@ -159,6 +168,10 @@ __global__ void __launch_bounds__(128) gather_blend_ms_kernel(const GatherBlendM
   gather_blend_body(p);
 }
 __global__ void __launch_bounds__(128) gather_blend_anc_kernel(const GatherBlendAncParams p) {
+  GB_PUBLISH_AND_WAIT(p);
+  gather_blend_body(p);
+}
+__global__ void __launch_bounds__(128) gather_blend_unipc_kernel(const GatherBlendUniPCParams p) {
   GB_PUBLISH_AND_WAIT(p);
   gather_blend_body(p);
 }
@@ -256,5 +269,32 @@ extern "C" int rtti_gather_blend_step_anc(const void* const* peer_slots, void* c
   p.s_up = s_up; p.z = (const __half*)z; p.z_ref = (const __half*)z_ref;
   const long long nv = n / 8;
   gather_blend_anc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+extern "C" int rtti_gather_blend_step_unipc(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                            const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                            long long n, float guidance, void* eps_out, const void* latents,
+                                            void* latents_out, const void* latents_ref, void* latents_ref_out,
+                                            float hx, float he, float ux, float ul, float u0, float u1, float u2,
+                                            float vx, float v0, float v1, const float* xl, const float* m1,
+                                            const float* m2, float* m_out, float* xl_out, const float* xl_ref,
+                                            const float* m1_ref, const float* m2_ref, float* m_out_ref,
+                                            float* xl_out_ref, unsigned int step_id, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  GatherBlendUniPCParams p{};
+  int rc = gather_blend_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                             eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = unipc_step_args(ul, u1, u2, v1, xl, m1, m2, m_out, xl_out);
+  if (rc == RTTI_OK && latents_ref != nullptr)
+    rc = unipc_step_args(ul, u1, u2, v1, xl_ref, m1_ref, m2_ref, m_out_ref, xl_out_ref);
+  if (rc == RTTI_OK && (((uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out |
+                         (uintptr_t)latents_ref | (uintptr_t)latents_ref_out) & 15))
+    rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.up = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl, m1, m2, m_out, xl_out};
+  p.up_ref = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl_ref, m1_ref, m2_ref, m_out_ref, xl_out_ref};
+  const long long nv = n / 8;
+  gather_blend_unipc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

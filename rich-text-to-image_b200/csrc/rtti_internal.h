@@ -35,6 +35,16 @@ inline int anc_step_args(float s_up, const void* z) {
   return ((uintptr_t)z & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
 }
 
+// the buffers of a UniPC blend step: m_out and xl_out required; xl required when ul != 0, m1 when u1 or v1 != 0, m2
+// when u2 != 0; all 16-byte aligned
+inline int unipc_step_args(float ul, float u1, float u2, float v1, const float* xl, const float* m1, const float* m2,
+                           const float* m_out, const float* xl_out) {
+  if (!m_out || !xl_out || (ul != 0.f && !xl) || ((u1 != 0.f || v1 != 0.f) && !m1) || (u2 != 0.f && !m2))
+    return RTTI_ERR_ARG;
+  return (((uintptr_t)xl | (uintptr_t)m1 | (uintptr_t)m2 | (uintptr_t)m_out | (uintptr_t)xl_out) & 15) ? RTTI_ERR_ALIGN
+                                                                                                      : RTTI_OK;
+}
+
 #ifdef __CUDACC__
 // GroupNorm statistics of a set of values as (count n, mean, m2 = sum of squared deviations from the mean), merged with
 // the pairwise update of Chan, Golub & LeVeque. Unlike a one-pass E[x^2] - E[x]^2 in fp32, which loses about
@@ -127,6 +137,53 @@ __device__ __forceinline__ void anc_step8(const AncStep& s, long long v, const f
       x[2 * i + 1] = fmaf(t.y, s.s_up, x[2 * i + 1]);
     }
   }
+}
+
+// The UniPC (bh2, order 2) update in data-prediction form (schedulers.py, UniPCMultistepScheduler.unipc_coeffs):
+//   m  = hx * x + he * eps                                   written to m_out
+//   xc = ux * x + ul * xl + u0 * m + u1 * m1 + u2 * m2       the corrected sample, written to xl_out
+//   x' = vx * xc + v0 * m + v1 * m1                          the predictor, rounded to fp16 by the caller
+// with xl = xc of the previous step, m1 / m2 = m of the previous two steps, fp32 [n] each. A history is read (128-bit)
+// only when one of its coefficients is non-zero; an unread one counts as 0. m_out may alias m2 and xl_out may alias xl:
+// each thread loads its 8 elements of every history before it stores any.
+struct UniPCStep {
+  float hx, he, ux, ul, u0, u1, u2, vx, v0, v1;
+  const float* xl;
+  const float* m1;
+  const float* m2;
+  float* m_out;
+  float* xl_out;
+};
+
+__device__ __forceinline__ void ld8f(const float* p, float* f) {
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+__device__ __forceinline__ void st8f(float* p, const float* f) {
+  *reinterpret_cast<float4*>(p) = make_float4(f[0], f[1], f[2], f[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(f[4], f[5], f[6], f[7]);
+}
+
+__device__ __forceinline__ void unipc_step8(const UniPCStep& s, long long v, const float* e16, float* x) {
+  float l[8], a[8], b[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { l[i] = 0.f; a[i] = 0.f; b[i] = 0.f; }
+  if (s.ul != 0.f) ld8f(s.xl + v * 8, l);
+  if (s.u1 != 0.f || s.v1 != 0.f) ld8f(s.m1 + v * 8, a);
+  if (s.u2 != 0.f) ld8f(s.m2 + v * 8, b);
+  float m[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    m[i] = fmaf(s.he, e16[i], s.hx * x[i]);
+    float c = fmaf(s.u0, m[i], s.ux * x[i]);
+    c = fmaf(s.ul, l[i], c);
+    c = fmaf(s.u1, a[i], c);
+    c = fmaf(s.u2, b[i], c);
+    l[i] = c;
+    x[i] = fmaf(s.v1, a[i], fmaf(s.v0, m[i], s.vx * c));
+  }
+  st8f(s.m_out + v * 8, m);
+  st8f(s.xl_out + v * 8, l);
 }
 
 // fixed-order tree over the 32 lanes of a warp; lane 0 ends with the statistics of every lane

@@ -271,6 +271,54 @@ class AncestralStep:
         return a + ([_ptr(self.z_ref)] if ref else [])
 
 
+class UniPCHistory:
+    """The UniPC state of one trajectory: three fp32 [n] buffers, xl (the corrected sample of the last step) and the x0
+    predictions of the last two steps, m1 (newest) and m2. A step writes its m over m2 and its corrected sample over
+    xl; `rotate()` after the step makes that m the new m1."""
+
+    def __init__(self, n, device):
+        self.xl, self.m1, self.m2 = (torch.empty(n, dtype=torch.float32, device=device) for _ in range(3))
+
+    def rotate(self):
+        self.m1, self.m2 = self.m2, self.m1
+
+
+class UniPCStep:
+    """The UniPC update of one blend call: `coeffs` (schedulers.UniPCCoeffs) and the fp32 [n] buffers of one trajectory,
+    (xl, m1, m2, m_out, xl_out): xl read when ul != 0, m1 when u1 or v1 != 0, m2 when u2 != 0; m_out (may be m2) and
+    xl_out (may be xl) written. `ref`: the same five buffers of the reference-latent trajectory (gather_blend_step only).
+    `UniPCStep.of(coeffs, hist, hist_ref)` steps UniPCHistory objects in place (call their rotate() afterwards)."""
+
+    def __init__(self, coeffs, xl, m1, m2, m_out, xl_out, ref=None):
+        self.coeffs = tuple(float(c) for c in coeffs)
+        self.bufs = (xl, m1, m2, m_out, xl_out)
+        self.ref = tuple(ref) if ref is not None else None
+
+    @classmethod
+    def of(cls, coeffs, hist, hist_ref=None):
+        b = lambda h: (h.xl, h.m1, h.m2, h.m2, h.xl)
+        return cls(coeffs, *b(hist), ref=b(hist_ref) if hist_ref is not None else None)
+
+    def _check(self, n, ref):
+        _, _, _, ul, _, u1, u2, _, _, v1 = self.coeffs
+        needed = (ul != 0.0, u1 != 0.0 or v1 != 0.0, u2 != 0.0, True, True)
+        names = ("xl", "m1", "m2", "m_out", "xl_out")
+        sets = [self.bufs] + ([self.ref or (None,) * 5] if ref else [])
+        for bufs in sets:
+            for t, need, name in zip(bufs, needed, names):
+                if t is None:
+                    if need:
+                        raise _lib.RttiError(f"UniPC blend: {name} is required")
+                    continue
+                _req(t, torch.float32, name)
+                if not t.is_contiguous() or t.numel() != n:
+                    raise _lib.RttiError(f"UniPC blend: {name} must be a contiguous fp32 tensor of {n} elements")
+
+    def args(self, ref=False):
+        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(t) for t in self.bufs]
+        return a + ([_ptr(t) for t in (self.ref or (None,) * 5)] if ref else [])
+
+
 def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0,
                      step=None):
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
@@ -279,7 +327,9 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     (rtti_region_blend_cfg_rescale); phi == 0 runs rtti_region_blend_cfg.
     step: a MultistepStep — the latents (required then) take the DDIM / DPM-Solver++ update instead of the Euler one
     (rtti_region_blend_cfg_ms / rtti_region_blend_cfg_rescale_ms; dt_sigma is not used); an AncestralStep — the
-    Euler Ancestral update (rtti_region_blend_cfg_anc / rtti_region_blend_cfg_rescale_anc; dt_sigma is not used)."""
+    Euler Ancestral update (rtti_region_blend_cfg_anc / rtti_region_blend_cfg_rescale_anc; dt_sigma is not used); a
+    UniPCStep — the UniPC update (rtti_region_blend_cfg_unipc / rtti_region_blend_cfg_rescale_unipc; dt_sigma is not
+    used)."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -290,7 +340,20 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    if isinstance(step, AncestralStep):
+    if isinstance(step, UniPCStep):
+        if latents is None:
+            raise _lib.RttiError("region_blend_cfg: a UniPC step needs the latents")
+        step._check(n, False)
+        if guidance_rescale == 0.0:
+            rc = lib.rtti_region_blend_cfg_unipc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                 _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_unipc")
+        else:
+            rc = lib.rtti_region_blend_cfg_rescale_unipc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                         _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
+                                                         float(guidance_rescale), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_rescale_unipc")
+    elif isinstance(step, AncestralStep):
         if latents is None:
             raise _lib.RttiError("region_blend_cfg: an ancestral step needs the latents")
         step._check(n, False)
@@ -399,7 +462,8 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     step: a MultistepStep (with d_prev_ref / d_out_ref when latents_ref is given) — the DDIM / DPM-Solver++ update
     instead of the Euler one (rtti_gather_blend_step_ms / rtti_gather_blend_step_rescale_ms); an AncestralStep (with
     z_ref when latents_ref is given) — the Euler Ancestral update (rtti_gather_blend_step_anc /
-    rtti_gather_blend_step_rescale_anc).
+    rtti_gather_blend_step_rescale_anc); a UniPCStep (with `ref` when latents_ref is given) — the UniPC update
+    (rtti_gather_blend_step_unipc / rtti_gather_blend_step_rescale_unipc).
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
@@ -410,7 +474,17 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    if isinstance(step, AncestralStep):
+    if isinstance(step, UniPCStep):
+        step._check(n, latents_ref is not None)
+        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
+                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
+        args += step.args(ref=True) + [int(step_id)]
+        if guidance_rescale == 0.0:
+            _lib.check(lib.rtti_gather_blend_step_unipc(*args, _stream()), "rtti_gather_blend_step_unipc")
+        else:
+            _lib.check(lib.rtti_gather_blend_step_rescale_unipc(*args, float(guidance_rescale), _stream()),
+                       "rtti_gather_blend_step_rescale_unipc")
+    elif isinstance(step, AncestralStep):
         step._check(n, latents_ref is not None)
         args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
                 float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]

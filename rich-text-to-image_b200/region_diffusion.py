@@ -9,7 +9,8 @@ capture that overwrites instead of accumulating, :423), executed as one batched 
 
 `.scheduler` is PLMS (PNDMScheduler) by default and steps on the host; DDIMScheduler and DPMSolverMultistepScheduler
 (schedulers.py) step inside the fused blend kernels (rtti_region_blend_cfg_ms), with one fp32 history of the x0
-prediction per trajectory.
+prediction per trajectory; UniPCMultistepScheduler steps inside rtti_region_blend_cfg_unipc, with three fp32 histories
+per trajectory (ops.UniPCHistory).
 """
 import math
 from typing import Optional
@@ -19,7 +20,7 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers, SelfAttentionLayers
-from .schedulers import MULTISTEP_SCHEDULERS, PNDMScheduler
+from .schedulers import MULTISTEP_SCHEDULERS, PNDMScheduler, UniPCMultistepScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -143,6 +144,10 @@ class RegionDiffusion:
         if multistep:   # one x0-prediction history per trajectory (both are stepped on every step)
             d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev)
             d_hist_ref = torch.empty_like(d_hist) if inject else None
+        unipc = isinstance(self.scheduler, UniPCMultistepScheduler)
+        if unipc:       # one UniPC state per trajectory (both are stepped on every step)
+            up_hist = ops.UniPCHistory(latents.numel(), dev)
+            up_hist_ref = ops.UniPCHistory(latents.numel(), dev) if inject else None
         for i, t in enumerate(timesteps):
             feat_inject_step = bool(int(t) > (1 - inject_selfattn) * 1000)                                   # :104
             background_inject_step = (i == int(inject_background * n_t)) and inject_background > 0           # :105
@@ -172,6 +177,18 @@ class RegionDiffusion:
                                                           [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale,
                                                           latents=latents_ref.contiguous(),
                                                           step=ops.MultistepStep(c, d_hist_ref, d_hist_ref))
+            elif unipc:
+                c = self.scheduler.unipc_coeffs(i)
+                noise_pred, latents = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks,
+                                                           guidance_scale, latents=latents.contiguous(),
+                                                           step=ops.UniPCStep.of(c, up_hist))
+                up_hist.rotate()
+                if inject:
+                    _, latents_ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
+                                                          [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale,
+                                                          latents=latents_ref.contiguous(),
+                                                          step=ops.UniPCStep.of(c, up_hist_ref))
+                    up_hist_ref.rotate()
             else:
                 noise_pred = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks, guidance_scale)  # :119-132
                 if inject:                                                                                  # :134-143
@@ -205,6 +222,7 @@ class RegionDiffusion:
         ones = torch.ones(1, latents[0].numel(), dtype=torch.float32, device=dev)
         multistep = isinstance(self.scheduler, MULTISTEP_SCHEDULERS)
         d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev) if multistep else None
+        up_hist = ops.UniPCHistory(latents.numel(), dev) if isinstance(self.scheduler, UniPCMultistepScheduler) else None
         for i, t in enumerate(self.scheduler.timesteps):
             x = latents.expand(2, -1, -1, -1)
             ctrl = RegionControl(capture=self._capture, capture_row=1, kv_cache=kv)
@@ -213,6 +231,12 @@ class RegionDiffusion:
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(),
                                                   step=ops.MultistepStep(self.scheduler.step_coeffs(i), d_hist, d_hist))
+                continue
+            if up_hist is not None:
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=latents.contiguous(),
+                                                  step=ops.UniPCStep.of(self.scheduler.unipc_coeffs(i), up_hist))
+                up_hist.rotate()
                 continue
             noise_pred = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale)
             latents = self.scheduler.step(noise_pred, t, latents)["prev_sample"].to(torch.float16)

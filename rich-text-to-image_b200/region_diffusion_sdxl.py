@@ -9,8 +9,9 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
     reference latent, the input; the hook choreography becomes a RegionControl;
   * region blend + CFG (+ guidance rescale) + scheduler update is one kernel (rtti_region_blend_cfg, or
     rtti_region_blend_cfg_rescale with guidance_rescale > 0; their "_ms" forms for DDIM / DPM-Solver++(2M), which
-    keep one fp32 history of the x0 prediction per trajectory, and "_anc" forms for Euler Ancestral, which add the
-    noise drawn for the step); colour-guidance loss fwd/bwd,
+    keep one fp32 history of the x0 prediction per trajectory, "_anc" forms for Euler Ancestral, which add the
+    noise drawn for the step, and "_unipc" forms for UniPC, which keep three fp32 histories per trajectory);
+    colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
     per-pass noise predictions are all-gathered before the (replicated, deterministic) blend.
@@ -23,7 +24,8 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
-from .schedulers import MULTISTEP_SCHEDULERS, DDIMScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler
+from .schedulers import (MULTISTEP_SCHEDULERS, DDIMScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
+                         UniPCMultistepScheduler)
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -35,8 +37,11 @@ def _rescale_phi(guidance_scale, guidance_rescale):
 
 def _step_kind(scheduler):
     """The fused update a scheduler runs as: "euler" (EulerDiscreteScheduler), "ancestral"
-    (EulerAncestralDiscreteScheduler: the Euler update plus the noise term, ancestral_coeffs) or "multistep"
-    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs). Any other scheduler has no fused update here."""
+    (EulerAncestralDiscreteScheduler: the Euler update plus the noise term, ancestral_coeffs), "multistep"
+    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs) or "unipc" (UniPCMultistepScheduler, unipc_coeffs). Any
+    other scheduler has no fused update here."""
+    if isinstance(scheduler, UniPCMultistepScheduler):
+        return "unipc"
     if isinstance(scheduler, EulerAncestralDiscreteScheduler):
         return "ancestral"
     if isinstance(scheduler, EulerDiscreteScheduler):
@@ -44,8 +49,8 @@ def _step_kind(scheduler):
     if isinstance(scheduler, MULTISTEP_SCHEDULERS):
         return "multistep"
     raise TypeError(f"RegionDiffusionXL: unsupported scheduler {type(scheduler).__name__}; supported: "
-                    "EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler "
-                    "(rtti_b200.schedulers)")
+                    "EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler, "
+                    "UniPCMultistepScheduler (rtti_b200.schedulers)")
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -210,12 +215,15 @@ class RegionDiffusionXL:
         base prompt last (sample.py:107); embeddings may be passed instead of text. `guidance_rescale` (applied when
         guidance_scale > 1) rescales the CFG prediction as diffusers' rescale_noise_cfg in both passes; the reference
         implements it for the plain pass only (:903-905) and raises NotImplementedError in the rich-text pass (:827-830).
-        `self.scheduler` may be EulerDiscreteScheduler, DDIMScheduler or DPMSolverMultistepScheduler (schedulers.py);
-        `eta` > 0 (stochastic DDIM, which the reference's plain pass forwards to DDIM) is not implemented.
-        With a multistep scheduler the rich-text pass keeps one history per trajectory: where the reference steps the
-        reference latents jointly with the main latents only on a prefix of the steps (inject_selfattn = 0,
+        `self.scheduler` may be EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler,
+        DPMSolverMultistepScheduler or UniPCMultistepScheduler (schedulers.py); `eta` > 0 (stochastic DDIM, which the
+        reference's plain pass forwards to DDIM) is not implemented.
+        With a multistep or UniPC scheduler the rich-text pass keeps one history per trajectory: where the reference
+        steps the reference latents jointly with the main latents only on a prefix of the steps (inject_selfattn = 0,
         0 < inject_background < 1, :831-846) and then steps the main latents alone, the main latents keep their own
-        history here instead of continuing a batch-2 one.
+        history here instead of continuing a batch-2 one. UniPC's corrector restarts from its own last corrected
+        sample, so colour guidance and background injection reach its next update only through the x0 prediction of
+        the next step, as in the reference with UniPC assigned to its scheduler.
         With EulerAncestralDiscreteScheduler the noise z of each step is drawn as diffusers' randn_tensor draws it, fp16,
         from `generator` when one is given (on its device: a CPU generator draws on the CPU), otherwise from the global
         RNG of the sampling device. The plain pass draws [1, ...] per step, as the reference does. The rich-text pass
@@ -272,7 +280,8 @@ class RegionDiffusionXL:
                     guidance_rescale=0.0, generator=None):
         """:879-914 — CFG batch [uncond, cond]; with capture armed the attention kernels accumulate the maps.
         guidance_rescale rescales the CFG prediction inside the blend kernel (:903-905). A multistep scheduler: the UNet
-        sees the latents unscaled and the blend kernel takes the step_coeffs(i) update. Euler Ancestral: the UNet input
+        sees the latents unscaled and the blend kernel takes the step_coeffs(i) update; UniPC likewise, with
+        unipc_coeffs(i) and three histories (ops.UniPCHistory). Euler Ancestral: the UNet input
         is scaled as for Euler and the blend kernel adds s_up z, z [1, ...] drawn from `generator` after the UNet pass,
         as the reference's step draws it (:908)."""
         phi = _rescale_phi(guidance_scale, guidance_rescale)
@@ -283,8 +292,9 @@ class RegionDiffusionXL:
         kind = _step_kind(self.scheduler)
         multistep = kind == "multistep"
         d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=latents.device) if multistep else None
+        up_hist = ops.UniPCHistory(latents.numel(), latents.device) if kind == "unipc" else None
         for i, t in enumerate(timesteps):
-            if multistep:
+            if multistep or up_hist is not None:
                 x = latents.expand(2, -1, -1, -1)
             else:
                 sigma = self.scheduler.sigma(t)
@@ -298,6 +308,11 @@ class RegionDiffusionXL:
                 step = ops.MultistepStep(self.scheduler.step_coeffs(i), d_hist, d_hist)
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(), guidance_rescale=phi, step=step)
+            elif up_hist is not None:
+                step = ops.UniPCStep.of(self.scheduler.unipc_coeffs(i), up_hist)
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=latents.contiguous(), guidance_rescale=phi, step=step)
+                up_hist.rotate()
             elif kind == "ancestral":
                 dt, s_up = self.scheduler.ancestral_coeffs(i)
                 z = self.scheduler.noise(tuple(latents.shape), generator, latents.device)
@@ -362,11 +377,14 @@ class RegionDiffusionXL:
         st.noise_pred = None
         # multistep schedulers: one fp32 history of the x0 prediction per trajectory (main, reference)
         kind = _step_kind(self.scheduler)
-        st.multistep, st.ancestral = kind == "multistep", kind == "ancestral"
+        st.multistep, st.ancestral, st.unipc = kind == "multistep", kind == "ancestral", kind == "unipc"
         st.generator = generator
         n = latents.numel()
         st.d_hist = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep else None
         st.d_hist_ref = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep and inject else None
+        # UniPC: one state of three fp32 buffers per trajectory
+        st.up_hist = ops.UniPCHistory(n, dev) if st.unipc else None
+        st.up_hist_ref = ops.UniPCHistory(n, dev) if st.unipc and inject else None
         return st
 
     def _unet_pass(self, st, x, t, local, feat_inject_step):
@@ -461,7 +479,7 @@ class RegionDiffusionXL:
         passes, kind, plan, N = st.passes, st.kind, st.plan, st.N
         feat_inject_step = bool(float(t) > (1 - st.inject_selfattn) * 1000)            # :782
         background_inject_step = i < st.inject_background * st.n_t                      # :783
-        if st.multistep:   # scale_model_input is the identity
+        if st.multistep or st.unipc:   # scale_model_input is the identity
             scale = None
         else:
             sigma = self.scheduler.sigma(t)
@@ -493,6 +511,12 @@ class RegionDiffusionXL:
             step = ops.MultistepStep(c, st.d_hist, st.d_hist, st.d_hist_ref, st.d_hist_ref)
             step_main = ops.MultistepStep(c, st.d_hist, st.d_hist)
             step_refl = ops.MultistepStep(c, st.d_hist_ref, st.d_hist_ref)
+        elif st.unipc:
+            c = self.scheduler.unipc_coeffs(i)
+            dt = 0.0
+            step = ops.UniPCStep.of(c, st.up_hist, st.up_hist_ref if step_ref else None)
+            step_main = ops.UniPCStep.of(c, st.up_hist)
+            step_refl = ops.UniPCStep.of(c, st.up_hist_ref) if step_ref else None
         elif st.ancestral:
             # the reference draws z in its scheduler step (:837-846): one [2, ...] draw when it steps both trajectories
             # as one batch (main first), [1, ...] otherwise; on CUDA one [2, n] draw differs from two [1, n] draws
@@ -539,6 +563,10 @@ class RegionDiffusionXL:
                                                          latents=st.latents_ref.contiguous(), dt_sigma=dt,
                                                          guidance_rescale=st.guidance_rescale,
                                                          step=step_refl)
+        if st.unipc:   # this step's x0 prediction becomes m1 of the next step
+            st.up_hist.rotate()
+            if step_ref:
+                st.up_hist_ref.rotate()
         if pe is not None:
             ev[2].record()
         if st.use_guidance and float(t) < st.tfd["guidance_start_step"]:                                  # :849

@@ -10,6 +10,8 @@ DDIMScheduler and DPMSolverMultistepScheduler (below) are the schedulers a diffu
 (`model.scheduler = DPMSolverMultistepScheduler(...)`); the samplers run them through the fused blend kernels with
 the per-step coefficients of `step_coeffs(i)`. EulerAncestralDiscreteScheduler ("Euler a", SDXL) adds fresh noise on
 every step; the SDXL sampler runs it through the fused blend kernels with `ancestral_coeffs(i)`.
+UniPCMultistepScheduler (bh2, order 2, the few-step sampler) runs through the fused blend kernels of both samplers
+with `unipc_coeffs(i)`.
 """
 import math
 from typing import NamedTuple
@@ -175,8 +177,9 @@ class _Configured:
 
 
 class _MultistepBase(_Configured):
-    """Shared VP-space conventions of DDIMScheduler and DPMSolverMultistepScheduler: scaled-linear betas, epsilon
-    prediction, init_noise_sigma = 1, scale_model_input = identity (the UNet sees the latents unscaled),
+    """Shared VP-space conventions of DDIMScheduler, DPMSolverMultistepScheduler and UniPCMultistepScheduler:
+    scaled-linear betas, epsilon prediction, init_noise_sigma = 1, scale_model_input = identity (the UNet sees the
+    latents unscaled),
     alphas_cumprod = the same host fp32 tensor as the other schedulers (colour guidance's predict_x0), host int64
     timesteps. Write a_t = alphas_cumprod[t], alpha_t = sqrt(a_t), sigma_t = sqrt(1 - a_t),
     lambda_t = log alpha_t - log sigma_t."""
@@ -290,6 +293,130 @@ class DPMSolverMultistepScheduler(_MultistepBase):
 
 
 MULTISTEP_SCHEDULERS = (DDIMScheduler, DPMSolverMultistepScheduler)
+
+
+# ---------------------------------------------------------------------------------------------------- UniPC
+class UniPCCoeffs(NamedTuple):
+    """One step of UniPC (bh2, order 2) in data-prediction form (float64, host):
+        m  = hx * x + he * eps                                  (x0 prediction of this step)
+        xc = ux * x + ul * xl + u0 * m + u1 * m1 + u2 * m2      (corrected sample; xl = xc of the previous step,
+                                                                  m1 / m2 = m of the previous two steps)
+        x' = vx * xc + v0 * m + v1 * m1                         (predictor)
+    The blend kernels' UniPC entry points (rtti_*_unipc) evaluate exactly this with eps = the fp16-rounded prediction."""
+    hx: float
+    he: float
+    ux: float
+    ul: float
+    u0: float
+    u1: float
+    u2: float
+    vx: float
+    v0: float
+    v1: float
+
+
+class UniPCMultistepScheduler(_MultistepBase):
+    """UniPC: solver_type="bh2", solver_order=2, predict_x0=True, lower_order_final=True, no corrector disabled, no
+    solver_p, epsilon prediction — the defaults of diffusers 0.18.2 (`schedulers/scheduling_unipc_multistep.py`) with
+    the SD1.5 / SDXL betas, restated. PARITY UNPINNED: that source is not available here; the conventions below are the
+    definition. Timesteps: those of DPMSolverMultistepScheduler. Step i goes from t = ts[i] to s = ts[i+1] (s = 0 on the
+    last step); m_i = (x_i - sigma_t eps_i) / alpha_t, with x_i the latents the UNet saw at step i.
+      orders: predictor p_i = min(2, n - i, i + 1); corrector at i >= 1 of order c_i = p_{i-1}
+      corrector (UniC), i >= 1, t' = ts[i-1]: h = lambda_t - lambda_t', hh = -h, B = phi = expm1(hh),
+        x^ = (sigma_t / sigma_t') xc_{i-1} - alpha_t phi m_{i-1}
+        c_i = 1: xc_i = x^ - alpha_t B (m_i - m_{i-1}) / 2
+        c_i = 2: r = (lambda_{ts[i-2]} - lambda_t') / h, D = (m_{i-2} - m_{i-1}) / r, (rho0, rho1) solves
+                 [[1, 1], [r, 1]] rho = [g1, g2], g1 = (phi/hh - 1) / B, g2 = 2 ((phi/hh - 1)/hh - 1/2) / B;
+                 xc_i = x^ - alpha_t B (rho0 D + rho1 (m_i - m_{i-1}))
+        step 0: xc_0 = x_0
+      predictor (UniP): h = lambda_s - lambda_t, hh, B, phi as above,
+        x_{i+1} = (sigma_s / sigma_t) xc_i - alpha_s phi m_i - [p_i = 2] alpha_s B (m_{i-1} - m_i) / (2 r'),
+        r' = (lambda_{ts[i-1]} - lambda_t) / h
+    The corrector restarts from its own xc_{i-1}, so the current latents reach it only through m_i: whatever a sampling
+    loop does to the latents between two steps (colour guidance, background injection) acts on the next update through
+    the x0 prediction alone. The samplers run it through the fused blend kernels with the coefficients of
+    `unipc_coeffs(i)` and three fp32 histories per trajectory (ops.UniPCHistory)."""
+    _defaults = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                     trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                     dynamic_thresholding_ratio=0.995, sample_max_value=1.0, predict_x0=True, solver_type="bh2",
+                     lower_order_final=True, disable_corrector=[], solver_p=None, use_karras_sigmas=False,
+                     timestep_spacing="linspace", steps_offset=1)
+    _unsupported = dict(trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                        predict_x0=True, solver_type="bh2", lower_order_final=True, disable_corrector=[], solver_p=None,
+                        use_karras_sigmas=False, timestep_spacing="linspace")
+
+    def __init__(self, **kw):
+        if kw.get("disable_corrector") is not None:
+            kw["disable_corrector"] = list(kw["disable_corrector"])
+        if kw.get("solver_type") in ("midpoint", "heun", "logrho"):
+            kw["solver_type"] = "bh2"   # as diffusers does, so that from_config(DPMSolverMultistepScheduler) works
+        super().__init__(**kw)
+        self._xl = self._m1 = self._m2 = None
+
+    def set_timesteps(self, num_inference_steps, device=None):
+        DPMSolverMultistepScheduler.set_timesteps(self, num_inference_steps, device)
+        self._xl = self._m1 = self._m2 = None
+
+    def orders(self, i):
+        """(predictor order p_i, corrector order c_i; 0 at step 0, which has no corrector)."""
+        n = len(self.timesteps_host)
+        p = lambda k: min(2, n - k, k + 1)
+        return p(i), (p(i - 1) if i > 0 else 0)
+
+    def unipc_coeffs(self, i):
+        ts, n = self.timesteps_host, len(self.timesteps_host)
+        al, sg, lam = self._alpha, self._sigma, self._lambda
+        t = int(ts[i])
+        s = 0 if i == n - 1 else int(ts[i + 1])
+        p, c = self.orders(i)
+        hx, he = 1.0 / al[t], -sg[t] / al[t]
+        if c == 0:
+            ux, ul, u0, u1, u2 = 1.0, 0.0, 0.0, 0.0, 0.0
+        else:
+            tp = int(ts[i - 1])
+            h = lam[t] - lam[tp]
+            hh = -h
+            phi = math.expm1(hh)
+            a = al[t] * phi                      # alpha_t * B (bh2: B = phi)
+            ux, ul = 0.0, sg[t] / sg[tp]
+            if c == 1:
+                rho0, rho1, r = 0.0, 0.5, 1.0
+            else:
+                r = (lam[int(ts[i - 2])] - lam[tp]) / h
+                g1 = (phi / hh - 1.0) / phi
+                g2 = 2.0 * ((phi / hh - 1.0) / hh - 0.5) / phi
+                rho0 = (g1 - g2) / (1.0 - r)
+                rho1 = g1 - rho0
+            # xc = ul xl - a m1 - a (rho0 (m2 - m1) / r + rho1 (m - m1))
+            u0, u1, u2 = -a * rho1, -a * (1.0 - rho0 / r - rho1), -a * rho0 / r
+        h = lam[s] - lam[t]
+        phi = math.expm1(-h)
+        b = al[s] * phi
+        vx = sg[s] / sg[t]
+        if p == 1:
+            v0, v1 = -b, 0.0
+        else:
+            rp = (lam[int(ts[i - 1])] - lam[t]) / h
+            v0, v1 = -b + 0.5 * b / rp, -0.5 * b / rp
+        return UniPCCoeffs(*(float(v) for v in (hx, he, ux, ul, u0, u1, u2, vx, v0, v1)))
+
+    def step(self, model_output, timestep, sample, return_dict=True, **kw):
+        """Stateful torch form of unipc_coeffs (the samplers use the fused kernels instead), in the precision of
+        `sample` and at least fp32: keeps xc of the last step and m of the last two."""
+        c = self.unipc_coeffs(self.index_of(timestep))
+        dt = torch.promote_types(sample.dtype, torch.float32)
+        x, e = sample.to(dt), model_output.to(dt)
+        m = c.hx * x + c.he * e
+        xc = c.ux * x + c.u0 * m
+        for coef, hist in ((c.ul, self._xl), (c.u1, self._m1), (c.u2, self._m2)):
+            if coef != 0.0:
+                xc = xc + coef * hist
+        prev = c.vx * xc + c.v0 * m
+        if c.v1 != 0.0:
+            prev = prev + c.v1 * self._m1
+        self._xl, self._m1, self._m2 = xc, m, self._m1
+        prev = prev.to(sample.dtype)
+        return {"prev_sample": prev} if return_dict else (prev,)
 
 
 # ---------------------------------------------------------------------------------------------------- ancestral

@@ -4,8 +4,9 @@ capture, get_token_maps (twice: colour masks, region masks), rich-text pass.
 
 Extra flags: --load_path (LOCAL diffusers-format directory; there is no hub access in this environment),
 --synthetic (random weights + random prompt embeddings, for smoke runs without checkpoints) and
---scheduler {default,ddim,dpmpp_2m,euler_a} (default: PLMS for SD1.5, Euler for SDXL; DPM-Solver++(2M) is the usual
-choice at about 20 --sample_steps; euler_a, Euler Ancestral, is for SDXL / AnimeXL only).
+--scheduler {default,ddim,dpmpp_2m,euler_a,unipc} (default: PLMS for SD1.5, Euler for SDXL; DPM-Solver++(2M) is the
+usual choice at about 20 --sample_steps, UniPC the sampler built for 5-10; euler_a, Euler Ancestral, is for SDXL /
+AnimeXL only).
 """
 import argparse
 import json
@@ -22,7 +23,7 @@ from rtti_b200.attention_utils import get_token_maps  # noqa: E402
 from rtti_b200.region_diffusion import RegionDiffusion  # noqa: E402
 from rtti_b200.region_diffusion_sdxl import RegionDiffusionXL  # noqa: E402
 from rtti_b200.schedulers import (DDIMScheduler, DPMSolverMultistepScheduler,  # noqa: E402
-                                  EulerAncestralDiscreteScheduler)
+                                  EulerAncestralDiscreteScheduler, UniPCMultistepScheduler)
 from rtti_b200.richtext_utils import (get_attention_control_input, get_gradient_guidance_input,  # noqa: E402
                                       get_region_diffusion_input, parse_json, seed_everything)
 
@@ -49,7 +50,7 @@ def main(args, param):
     model = RegionDiffusionXL(load_path=args.load_path) if xl else RegionDiffusion("cuda", load_path=args.load_path)
     if args.scheduler != "default":
         model.scheduler = {"ddim": DDIMScheduler, "dpmpp_2m": DPMSolverMultistepScheduler,
-                           "euler_a": EulerAncestralDiscreteScheduler}[args.scheduler]()
+                           "euler_a": EulerAncestralDiscreteScheduler, "unipc": UniPCMultistepScheduler}[args.scheduler]()
 
     (base_prompt, style_prompts, footnote_prompts, footnote_targets, color_prompts, color_names, color_rgbs,
      sizes, use_grad_guidance) = parse_json(param["text_input"])
@@ -118,7 +119,8 @@ if __name__ == "__main__":
     p.add_argument("--num_segments", type=int, default=9)
     p.add_argument("--inject_background", type=float, default=0.0)
     p.add_argument("--load_path", type=str, default=None)
-    p.add_argument("--scheduler", type=str, default="default", choices=["default", "ddim", "dpmpp_2m", "euler_a"])
+    p.add_argument("--scheduler", type=str, default="default",
+                   choices=["default", "ddim", "dpmpp_2m", "euler_a", "unipc"])
     a = p.parse_args()
     res = 512 if a.model == "SD" else 1024
     main(a, {"text_input": json.loads(a.rich_text_json), "height": a.height or res, "width": a.width or res,
