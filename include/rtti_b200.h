@@ -197,6 +197,26 @@ int rtti_region_blend_cfg_rescale_unipc(const void* eps_uncond, const void* cons
                                         const float* m2, float* m_out, float* xl_out, float guidance_rescale,
                                         void* stream);
 
+/* Heun forms ("_heun") of the blend entry points, for Heun's method (rich-text-to-image_b200/schedulers.py,
+ * HeunDiscreteScheduler.heun_coeffs). They replace the scheduler step of models/region_diffusion_sdxl.py:837-846 and
+ * :908 with a HeunDiscreteScheduler assigned to the reference's scheduler. The blend, CFG and rescale arithmetic is
+ * that of the Euler form; the update of the latents is, in fp32,
+ *   x' = cx * x + ce * eps + cd * ds + cs * xs      (x' rounded to fp16)
+ * with x the fp16 latents, eps the fp16-rounded (rescaled) noise prediction written to eps_out, and xs[n] / ds[n] the
+ * fp16 latents and noise prediction of the last first stage: (cx, ce, cs, cd) = (1, dt, 0, 0) at a first stage,
+ * (0, dt/2, 1, dt/2) at a second. ds is read only when cd != 0 and xs only when cs != 0; with (1, dt, 0, 0) the result
+ * equals the Euler form's with dt_sigma = dt, bit for bit. latents and latents_out are required; xs is required when
+ * cs != 0 and ds when cd != 0, both 16-byte aligned when given. The other checks are those of the Euler form; on any
+ * error nothing is launched. */
+int rtti_region_blend_cfg_heun(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                               int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                               void* latents_out, float cx, float ce, float cs, float cd, const void* xs,
+                               const void* ds, void* stream);
+int rtti_region_blend_cfg_rescale_heun(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                       int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                       void* latents_out, float cx, float ce, float cs, float cd, const void* xs,
+                                       const void* ds, float guidance_rescale, void* stream);
+
 /* Colour-guidance loss forward + analytic backward w.r.t. the VAE decoder output.
  * Replaces models/region_diffusion_sdxl.py:857-865 (clamp, masked mean RGB, MSE*100, autograd of those).
  *   decoded [3, hw] fp32 (VAE output before /2+0.5), masks [n_colors, hw] fp32 (channel 0 of
@@ -337,6 +357,28 @@ int rtti_gather_blend_step_rescale_unipc(const void* const* peer_slots, void* co
                                          float* m_out, float* xl_out, const float* xl_ref, const float* m1_ref,
                                          const float* m2_ref, float* m_out_ref, float* xl_out_ref,
                                          unsigned int step_id, float guidance_rescale, void* stream);
+
+/* Heun forms of rtti_gather_blend_step / rtti_gather_blend_step_rescale (the update of rtti_region_blend_cfg_heun;
+ * they replace models/region_diffusion_sdxl.py:837-846 with a HeunDiscreteScheduler assigned to the reference's
+ * scheduler). The reference-latent trajectory, when latents_ref is given, is stepped with the same coefficients on its
+ * own saved state xs_ref / ds_ref (with the requirements of xs / ds). eps_ref_out[n], optional (null: not written;
+ * given without latents_ref: RTTI_ERR_ARG; 16-byte aligned), receives that trajectory's fp16-rounded (rescaled) noise
+ * prediction, the eps_out of the single-GPU form called on the C/D pair with one region and a mask of ones: its ds for
+ * the next second stage. For the same noise predictions the outputs equal those of the single-GPU forms bit for bit,
+ * whatever the world size. Same protocol and slot layout as the Euler forms. */
+int rtti_gather_blend_step_heun(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                                float guidance, void* eps_out, const void* latents, void* latents_out,
+                                const void* latents_ref, void* latents_ref_out, float cx, float ce, float cs, float cd,
+                                const void* xs, const void* ds, const void* xs_ref, const void* ds_ref,
+                                void* eps_ref_out, unsigned int step_id, void* stream);
+int rtti_gather_blend_step_rescale_heun(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                        const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                        long long n, float guidance, void* eps_out, const void* latents,
+                                        void* latents_out, const void* latents_ref, void* latents_ref_out, float cx,
+                                        float ce, float cs, float cd, const void* xs, const void* ds,
+                                        const void* xs_ref, const void* ds_ref, void* eps_ref_out,
+                                        unsigned int step_id, float guidance_rescale, void* stream);
 
 /* Stripe-parallel colour guidance (multi-GPU; new relative to the single-GPU reference, which back-propagates
  * through the batch-1 VAE decoder on one device: models/region_diffusion_sdxl.py:849-867). Every activation of

@@ -71,7 +71,14 @@ struct RescaleUniPCParams : RescaleParams {
   UniPCStep up, up_ref;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC update of the main (REF
+// the Heun form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory, and where the
+// reference trajectory's rescaled fp16 prediction goes (gather form only; null: not written)
+struct RescaleHeunParams : RescaleParams {
+  HeunStep hs, hs_ref;
+  __half* eps_ref_out;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun update of the main (REF
 // false) / reference (REF true) trajectory
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleParams& p, long long, const float* e16, float* x) {
@@ -90,6 +97,14 @@ template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleUniPCParams& p, long long v, const float* e16, float* x) {
   unipc_step8(REF ? p.up_ref : p.up, v, e16, x);
 }
+template <bool REF>
+__device__ __forceinline__ void rs_step(const RescaleHeunParams& p, long long v, const float* e16, float* x) {
+  heun_step8(REF ? p.hs_ref : p.hs, v, e16, x);
+}
+
+// the output of the reference trajectory's prediction: only the Heun form stores it (the ds of its first stage)
+__device__ __forceinline__ __half* rs_ref_eps(const RescaleParams&) { return nullptr; }
+__device__ __forceinline__ __half* rs_ref_eps(const RescaleHeunParams& p) { return p.eps_ref_out; }
 
 // (count, mean, m2) of eps_text and of eps_cfg over the same elements
 struct PairStats { int n; float mt, qt, mc, qc; };
@@ -258,7 +273,7 @@ __device__ __forceinline__ void blend_rescale_body(const P& p, float4* cfg_s, Re
   }
   rescale_job<PEER, false>(p, 0, p.n_regions, p.eps_out, p.latents, p.latents_out, cfg_s, sm);
   if (p.latents_ref != nullptr)
-    rescale_job<PEER, true>(p, p.n_regions + 1, 1, nullptr, p.latents_ref, p.latents_ref_out, cfg_s, sm);
+    rescale_job<PEER, true>(p, p.n_regions + 1, 1, rs_ref_eps(p), p.latents_ref, p.latents_ref_out, cfg_s, sm);
 }
 
 template <bool PEER>
@@ -293,6 +308,14 @@ __global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
   blend_rescale_body<PEER>(p, cfg_s, sm);
 }
 
+template <bool PEER>
+__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
+    blend_rescale_heun_kernel(const __grid_constant__ RescaleHeunParams p) {
+  extern __shared__ float4 cfg_s[];
+  __shared__ RescaleSmem sm;
+  blend_rescale_body<PEER>(p, cfg_s, sm);
+}
+
 // the kernel of each parameter type
 template <bool PEER>
 const void* rescale_kernel(const RescaleParams&) { return (const void*)blend_rescale_kernel<PEER>; }
@@ -302,6 +325,8 @@ template <bool PEER>
 const void* rescale_kernel(const RescaleAncParams&) { return (const void*)blend_rescale_anc_kernel<PEER>; }
 template <bool PEER>
 const void* rescale_kernel(const RescaleUniPCParams&) { return (const void*)blend_rescale_unipc_kernel<PEER>; }
+template <bool PEER>
+const void* rescale_kernel(const RescaleHeunParams&) { return (const void*)blend_rescale_heun_kernel<PEER>; }
 
 // threads per CTA and vectors per thread: a function of n only
 void rescale_plan(long long n, int& threads, int& vpt) {
@@ -327,6 +352,8 @@ int launch_rescale(P& p, void* stream) {
     blend_rescale_anc_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else if constexpr (std::is_same<P, RescaleUniPCParams>::value)
     blend_rescale_unipc_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
+  else if constexpr (std::is_same<P, RescaleHeunParams>::value)
+    blend_rescale_heun_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else
     blend_rescale_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
@@ -521,5 +548,44 @@ extern "C" int rtti_gather_blend_step_rescale_unipc(const void* const* peer_slot
   p.phi = guidance_rescale;
   p.up = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl, m1, m2, m_out, xl_out};
   p.up_ref = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl_ref, m1_ref, m2_ref, m_out_ref, xl_out_ref};
+  return launch_rescale<true>(p, stream);
+}
+
+extern "C" int rtti_region_blend_cfg_rescale_heun(const void* eps_uncond, const void* const* eps_region,
+                                                  const float* masks, int n_regions, long long n, float guidance,
+                                                  void* eps_out, const void* latents, void* latents_out, float cx,
+                                                  float ce, float cs, float cd, const void* xs, const void* ds,
+                                                  float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleHeunParams p{};
+  int rc = rescale_args(eps_uncond, eps_region, masks, n_regions, n, guidance, eps_out, latents, latents_out, p);
+  if (rc == RTTI_OK) rc = heun_step_args(cs, cd, xs, ds);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.hs = HeunStep{cx, ce, cs, cd, (const __half*)xs, (const __half*)ds};
+  return launch_rescale<false>(p, stream);
+}
+
+extern "C" int rtti_gather_blend_step_rescale_heun(const void* const* peer_slots, void* const* peer_flags, int world,
+                                                   int rank, const int* slot_owner, int n_slots, int n_regions,
+                                                   const float* masks, long long n, float guidance, void* eps_out,
+                                                   const void* latents, void* latents_out, const void* latents_ref,
+                                                   void* latents_ref_out, float cx, float ce, float cs, float cd,
+                                                   const void* xs, const void* ds, const void* xs_ref,
+                                                   const void* ds_ref, void* eps_ref_out, unsigned int step_id,
+                                                   float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  if (eps_ref_out != nullptr && latents_ref == nullptr) return RTTI_ERR_ARG;
+  RescaleHeunParams p{};
+  int rc = gather_rescale_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                               eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = heun_step_args(cs, cd, xs, ds);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = heun_step_args(cs, cd, xs_ref, ds_ref);
+  if (rc == RTTI_OK && ((uintptr_t)eps_ref_out & 15)) rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.hs = HeunStep{cx, ce, cs, cd, (const __half*)xs, (const __half*)ds};
+  p.hs_ref = HeunStep{cx, ce, cs, cd, (const __half*)xs_ref, (const __half*)ds_ref};
+  p.eps_ref_out = (__half*)eps_ref_out;
   return launch_rescale<true>(p, stream);
 }

@@ -343,8 +343,8 @@ __global__ void geglu_kernel(const __half* __restrict__ proj, __half* __restrict
 // ============================================================================ region blend + CFG
 struct BlendPtrs { const __half* eps[16]; };
 
-// step policies (rtti_internal.h): Euler, the multistep update of MsStep, the ancestral update of AncStep, or the UniPC
-// update of UniPCStep
+// step policies (rtti_internal.h): Euler, the multistep update of MsStep, the ancestral update of AncStep, the UniPC
+// update of UniPCStep, or the Heun update of HeunStep
 struct EulerStep { float dt_sigma; };
 __device__ __forceinline__ void apply_step(const EulerStep& s, long long, const float* e16, float* x) {
 #pragma unroll
@@ -355,6 +355,7 @@ __device__ __forceinline__ void apply_step(const AncStep& s, long long v, const 
 __device__ __forceinline__ void apply_step(const UniPCStep& s, long long v, const float* e16, float* x) {
   unipc_step8(s, v, e16, x);
 }
+__device__ __forceinline__ void apply_step(const HeunStep& s, long long v, const float* e16, float* x) { heun_step8(s, v, e16, x); }
 
 template <class Step>
 __device__ __forceinline__ void region_blend_body(const __half* __restrict__ eps_uncond, const BlendPtrs& ptrs,
@@ -419,6 +420,13 @@ __global__ void region_blend_unipc_kernel(const __half* __restrict__ eps_uncond,
                                           const float* __restrict__ masks, int n_regions, long long n, float guidance,
                                           __half* __restrict__ eps_out, const __half* __restrict__ latents,
                                           __half* __restrict__ latents_out, const UniPCStep st) {
+  region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
+}
+
+__global__ void region_blend_heun_kernel(const __half* __restrict__ eps_uncond, BlendPtrs ptrs,
+                                         const float* __restrict__ masks, int n_regions, long long n, float guidance,
+                                         __half* __restrict__ eps_out, const __half* __restrict__ latents,
+                                         __half* __restrict__ latents_out, const HeunStep st) {
   region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
 }
 
@@ -703,6 +711,22 @@ extern "C" int rtti_region_blend_cfg_unipc(const void* eps_uncond, const void* c
   region_blend_unipc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
       (__half*)latents_out, UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl, m1, m2, m_out, xl_out});
+  return ok_or_cuda();
+}
+
+extern "C" int rtti_region_blend_cfg_heun(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                          int n_regions, long long n, float guidance, void* eps_out,
+                                          const void* latents, void* latents_out, float cx, float ce, float cs,
+                                          float cd, const void* xs, const void* ds, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  BlendPtrs ptrs{};
+  int rc = region_blend_args(eps_uncond, eps_region, masks, n_regions, n, eps_out, latents, latents_out, ptrs);
+  if (rc == RTTI_OK) rc = heun_step_args(cs, cd, xs, ds);
+  if (rc != RTTI_OK) return rc;
+  const long long nv = n / 8;
+  region_blend_heun_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
+      (__half*)latents_out, HeunStep{cx, ce, cs, cd, (const __half*)xs, (const __half*)ds});
   return ok_or_cuda();
 }
 

@@ -74,7 +74,14 @@ struct GatherBlendUniPCParams : GatherBlendParams {
   UniPCStep up, up_ref;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC update of the main /
+// the Heun form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory, and where the
+// reference trajectory's fp16 prediction goes (null: not written)
+struct GatherBlendHeunParams : GatherBlendParams {
+  HeunStep hs, hs_ref;
+  __half* eps_ref_out;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun update of the main /
 // reference trajectory
 __device__ __forceinline__ void gb_step(const GatherBlendParams& p, bool, long long, const float* e16, float* x) {
 #pragma unroll
@@ -89,6 +96,15 @@ __device__ __forceinline__ void gb_step(const GatherBlendAncParams& p, bool ref,
 __device__ __forceinline__ void gb_step(const GatherBlendUniPCParams& p, bool ref, long long v, const float* e16,
                                         float* x) {
   unipc_step8(ref ? p.up_ref : p.up, v, e16, x);
+}
+__device__ __forceinline__ void gb_step(const GatherBlendHeunParams& p, bool ref, long long v, const float* e16, float* x) {
+  heun_step8(ref ? p.hs_ref : p.hs, v, e16, x);
+}
+
+// the reference trajectory's fp16 prediction: only the Heun form stores it (the ds of its first stage)
+__device__ __forceinline__ void gb_ref_eps(const GatherBlendParams&, long long, const H8&) {}
+__device__ __forceinline__ void gb_ref_eps(const GatherBlendHeunParams& p, long long v8, const H8& h) {
+  if (p.eps_ref_out != nullptr) *reinterpret_cast<H8*>(p.eps_ref_out + v8 * 8) = h;
 }
 
 // steps 1 and 2: publish this rank's step, wait for every peer it reads from. A macro rather than a function: written
@@ -152,7 +168,9 @@ __device__ __forceinline__ void gather_blend_body(const P& p) {
     up8(ld_peer(slot(p.n_regions + 2)), d);
 #pragma unroll
     for (int i = 0; i < 8; ++i) c[i] = c[i] + p.guidance * (d[i] - c[i]);
-    up8(pk8(c), e16);
+    const H8 ch = pk8(c);
+    gb_ref_eps(p, v8, ch);
+    up8(ch, e16);
     up8(*reinterpret_cast<const H8*>(p.latents_ref + v8 * 8), x);
     gb_step(p, true, v8, e16, x);
     *reinterpret_cast<H8*>(p.latents_ref_out + v8 * 8) = pk8(x);
@@ -172,6 +190,10 @@ __global__ void __launch_bounds__(128) gather_blend_anc_kernel(const GatherBlend
   gather_blend_body(p);
 }
 __global__ void __launch_bounds__(128) gather_blend_unipc_kernel(const GatherBlendUniPCParams p) {
+  GB_PUBLISH_AND_WAIT(p);
+  gather_blend_body(p);
+}
+__global__ void __launch_bounds__(128) gather_blend_heun_kernel(const GatherBlendHeunParams p) {
   GB_PUBLISH_AND_WAIT(p);
   gather_blend_body(p);
 }
@@ -296,5 +318,31 @@ extern "C" int rtti_gather_blend_step_unipc(const void* const* peer_slots, void*
   p.up_ref = UniPCStep{hx, he, ux, ul, u0, u1, u2, vx, v0, v1, xl_ref, m1_ref, m2_ref, m_out_ref, xl_out_ref};
   const long long nv = n / 8;
   gather_blend_unipc_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+extern "C" int rtti_gather_blend_step_heun(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                           const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                           long long n, float guidance, void* eps_out, const void* latents,
+                                           void* latents_out, const void* latents_ref, void* latents_ref_out, float cx,
+                                           float ce, float cs, float cd, const void* xs, const void* ds,
+                                           const void* xs_ref, const void* ds_ref, void* eps_ref_out,
+                                           unsigned int step_id, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  if (eps_ref_out != nullptr && latents_ref == nullptr) return RTTI_ERR_ARG;
+  GatherBlendHeunParams p{};
+  int rc = gather_blend_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                             eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = heun_step_args(cs, cd, xs, ds);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = heun_step_args(cs, cd, xs_ref, ds_ref);
+  if (rc == RTTI_OK && (((uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out |
+                         (uintptr_t)latents_ref | (uintptr_t)latents_ref_out | (uintptr_t)eps_ref_out) & 15))
+    rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.hs = HeunStep{cx, ce, cs, cd, (const __half*)xs, (const __half*)ds};
+  p.hs_ref = HeunStep{cx, ce, cs, cd, (const __half*)xs_ref, (const __half*)ds_ref};
+  p.eps_ref_out = (__half*)eps_ref_out;
+  const long long nv = n / 8;
+  gather_blend_heun_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

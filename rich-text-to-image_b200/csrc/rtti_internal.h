@@ -45,6 +45,12 @@ inline int unipc_step_args(float ul, float u1, float u2, float v1, const float* 
                                                                                                       : RTTI_OK;
 }
 
+// the saved state of a Heun blend step: xs required when cs != 0, ds when cd != 0; both 16-byte aligned
+inline int heun_step_args(float cs, float cd, const void* xs, const void* ds) {
+  if ((cs != 0.f && !xs) || (cd != 0.f && !ds)) return RTTI_ERR_ARG;
+  return (((uintptr_t)xs | (uintptr_t)ds) & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
+}
+
 #ifdef __CUDACC__
 // GroupNorm statistics of a set of values as (count n, mean, m2 = sum of squared deviations from the mean), merged with
 // the pairwise update of Chan, Golub & LeVeque. Unlike a one-pass E[x^2] - E[x]^2 in fp32, which loses about
@@ -184,6 +190,42 @@ __device__ __forceinline__ void unipc_step8(const UniPCStep& s, long long v, con
   }
   st8f(s.m_out + v * 8, m);
   st8f(s.xl_out + v * 8, l);
+}
+
+// The Heun update (schedulers.py, HeunDiscreteScheduler.heun_coeffs), in fp32:
+//   x' = cx * x + ce * eps + cd * ds + cs * xs
+// with xs / ds the fp16 [n] latents and stepped noise prediction saved at the first stage: (1, dt, 0, 0) at a first
+// stage, (0, dt/2, 1, dt/2) at a second. ds is read (128-bit) only when cd != 0 and xs only when cs != 0. The Euler
+// update is formed first (cx * x is exact for cx = 1), so a first stage gives the Euler bits with dt_sigma = ce; the
+// two dt/2 terms are summed before the latents xs are added.
+struct HeunStep {
+  float cx, ce, cs, cd;
+  const __half* xs;
+  const __half* ds;
+};
+
+__device__ __forceinline__ void heun_ld8(const __half* p, float* f) {
+  const uint4 u = *reinterpret_cast<const uint4*>(p);
+  const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) { const float2 t = __half22float2(h[i]); f[2 * i] = t.x; f[2 * i + 1] = t.y; }
+}
+
+__device__ __forceinline__ void heun_step8(const HeunStep& s, long long v, const float* e16, float* x) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], s.ce, s.cx * x[i]);
+  if (s.cd != 0.f) {
+    float d[8];
+    heun_ld8(s.ds + v * 8, d);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] = fmaf(d[i], s.cd, x[i]);
+  }
+  if (s.cs != 0.f) {
+    float p[8];
+    heun_ld8(s.xs + v * 8, p);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) x[i] = fmaf(p[i], s.cs, x[i]);
+  }
 }
 
 // fixed-order tree over the 32 lanes of a warp; lane 0 ends with the statistics of every lane

@@ -319,6 +319,41 @@ class UniPCStep:
         return a + ([_ptr(t) for t in (self.ref or (None,) * 5)] if ref else [])
 
 
+class HeunStep:
+    """The Heun update of one blend call: `coeffs` (cx, ce, cs, cd) from schedulers.HeunDiscreteScheduler.heun_coeffs,
+    x' = cx x + ce eps + cs xs + cd ds, with xs / ds the fp16 [n] latents and stepped noise prediction saved at the last
+    first stage (xs read when cs != 0, ds when cd != 0; may be None otherwise). xs_ref / ds_ref: the reference-latent
+    trajectory's; eps_ref_out: an fp16 [n] tensor that receives that trajectory's stepped prediction, or None
+    (gather_blend_step only)."""
+
+    def __init__(self, coeffs, xs, ds, xs_ref=None, ds_ref=None, eps_ref_out=None):
+        self.coeffs = tuple(float(c) for c in coeffs)
+        if len(self.coeffs) != 4:
+            raise _lib.RttiError(f"Heun blend: coeffs must be (cx, ce, cs, cd), got {len(self.coeffs)} values")
+        self.xs, self.ds, self.xs_ref, self.ds_ref, self.eps_ref_out = xs, ds, xs_ref, ds_ref, eps_ref_out
+
+    def _check(self, n, ref):
+        _, _, cs, cd = self.coeffs
+        items = [(self.xs, cs != 0.0, "xs"), (self.ds, cd != 0.0, "ds")]
+        if ref:
+            items += [(self.xs_ref, cs != 0.0, "xs_ref"), (self.ds_ref, cd != 0.0, "ds_ref"),
+                      (self.eps_ref_out, False, "eps_ref_out")]
+        elif self.eps_ref_out is not None:
+            raise _lib.RttiError("Heun blend: eps_ref_out needs the reference latents")
+        for t, need, name in items:
+            if t is None:
+                if need:
+                    raise _lib.RttiError(f"Heun blend: {name} is required")
+                continue
+            _req(t, _F16, name)
+            if not t.is_contiguous() or t.numel() != n:
+                raise _lib.RttiError(f"Heun blend: {name} must be a contiguous fp16 tensor of {n} elements")
+
+    def args(self, ref=False):
+        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(self.xs), _ptr(self.ds)]
+        return a + ([_ptr(self.xs_ref), _ptr(self.ds_ref), _ptr(self.eps_ref_out)] if ref else [])
+
+
 def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0,
                      step=None):
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
@@ -329,7 +364,8 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     (rtti_region_blend_cfg_ms / rtti_region_blend_cfg_rescale_ms; dt_sigma is not used); an AncestralStep — the
     Euler Ancestral update (rtti_region_blend_cfg_anc / rtti_region_blend_cfg_rescale_anc; dt_sigma is not used); a
     UniPCStep — the UniPC update (rtti_region_blend_cfg_unipc / rtti_region_blend_cfg_rescale_unipc; dt_sigma is not
-    used)."""
+    used); a HeunStep — the Heun update (rtti_region_blend_cfg_heun / rtti_region_blend_cfg_rescale_heun; dt_sigma is
+    not used, nor are xs_ref / ds_ref; eps_ref_out must be None)."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -340,7 +376,20 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    if isinstance(step, UniPCStep):
+    if isinstance(step, HeunStep):
+        if latents is None:
+            raise _lib.RttiError("region_blend_cfg: a Heun step needs the latents")
+        step._check(n, False)
+        if guidance_rescale == 0.0:
+            rc = lib.rtti_region_blend_cfg_heun(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_heun")
+        else:
+            rc = lib.rtti_region_blend_cfg_rescale_heun(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                        _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
+                                                        float(guidance_rescale), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_rescale_heun")
+    elif isinstance(step, UniPCStep):
         if latents is None:
             raise _lib.RttiError("region_blend_cfg: a UniPC step needs the latents")
         step._check(n, False)
@@ -463,7 +512,9 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     instead of the Euler one (rtti_gather_blend_step_ms / rtti_gather_blend_step_rescale_ms); an AncestralStep (with
     z_ref when latents_ref is given) — the Euler Ancestral update (rtti_gather_blend_step_anc /
     rtti_gather_blend_step_rescale_anc); a UniPCStep (with `ref` when latents_ref is given) — the UniPC update
-    (rtti_gather_blend_step_unipc / rtti_gather_blend_step_rescale_unipc).
+    (rtti_gather_blend_step_unipc / rtti_gather_blend_step_rescale_unipc); a HeunStep (with xs_ref / ds_ref, and
+    optionally eps_ref_out, when latents_ref is given) — the Heun update (rtti_gather_blend_step_heun /
+    rtti_gather_blend_step_rescale_heun).
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
@@ -474,7 +525,17 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    if isinstance(step, UniPCStep):
+    if isinstance(step, HeunStep):
+        step._check(n, latents_ref is not None)
+        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
+                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
+        args += step.args(ref=True) + [int(step_id)]
+        if guidance_rescale == 0.0:
+            _lib.check(lib.rtti_gather_blend_step_heun(*args, _stream()), "rtti_gather_blend_step_heun")
+        else:
+            _lib.check(lib.rtti_gather_blend_step_rescale_heun(*args, float(guidance_rescale), _stream()),
+                       "rtti_gather_blend_step_rescale_heun")
+    elif isinstance(step, UniPCStep):
         step._check(n, latents_ref is not None)
         args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
                 float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]

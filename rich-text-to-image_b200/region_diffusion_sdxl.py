@@ -10,7 +10,8 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
   * region blend + CFG (+ guidance rescale) + scheduler update is one kernel (rtti_region_blend_cfg, or
     rtti_region_blend_cfg_rescale with guidance_rescale > 0; their "_ms" forms for DDIM / DPM-Solver++(2M), which
     keep one fp32 history of the x0 prediction per trajectory, "_anc" forms for Euler Ancestral, which add the
-    noise drawn for the step, and "_unipc" forms for UniPC, which keep three fp32 histories per trajectory);
+    noise drawn for the step, "_unipc" forms for UniPC, which keep three fp32 histories per trajectory, and "_heun"
+    forms for Heun's method, which read the fp16 latents and prediction saved at the first stage);
     colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
@@ -25,7 +26,7 @@ import torch
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
 from .schedulers import (MULTISTEP_SCHEDULERS, DDIMScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
-                         UniPCMultistepScheduler)
+                         HeunDiscreteScheduler, UniPCMultistepScheduler)
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -38,8 +39,10 @@ def _rescale_phi(guidance_scale, guidance_rescale):
 def _step_kind(scheduler):
     """The fused update a scheduler runs as: "euler" (EulerDiscreteScheduler), "ancestral"
     (EulerAncestralDiscreteScheduler: the Euler update plus the noise term, ancestral_coeffs), "multistep"
-    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs) or "unipc" (UniPCMultistepScheduler, unipc_coeffs). Any
-    other scheduler has no fused update here."""
+    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs), "unipc" (UniPCMultistepScheduler, unipc_coeffs) or
+    "heun" (HeunDiscreteScheduler, heun_coeffs). Any other scheduler has no fused update here."""
+    if isinstance(scheduler, HeunDiscreteScheduler):
+        return "heun"
     if isinstance(scheduler, UniPCMultistepScheduler):
         return "unipc"
     if isinstance(scheduler, EulerAncestralDiscreteScheduler):
@@ -50,7 +53,7 @@ def _step_kind(scheduler):
         return "multistep"
     raise TypeError(f"RegionDiffusionXL: unsupported scheduler {type(scheduler).__name__}; supported: "
                     "EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler, "
-                    "UniPCMultistepScheduler (rtti_b200.schedulers)")
+                    "UniPCMultistepScheduler, HeunDiscreteScheduler (rtti_b200.schedulers)")
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -216,14 +219,20 @@ class RegionDiffusionXL:
         guidance_scale > 1) rescales the CFG prediction as diffusers' rescale_noise_cfg in both passes; the reference
         implements it for the plain pass only (:903-905) and raises NotImplementedError in the rich-text pass (:827-830).
         `self.scheduler` may be EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler,
-        DPMSolverMultistepScheduler or UniPCMultistepScheduler (schedulers.py); `eta` > 0 (stochastic DDIM, which the
-        reference's plain pass forwards to DDIM) is not implemented.
+        DPMSolverMultistepScheduler, UniPCMultistepScheduler or HeunDiscreteScheduler (schedulers.py); `eta` > 0
+        (stochastic DDIM, which the reference's plain pass forwards to DDIM) is not implemented.
         With a multistep or UniPC scheduler the rich-text pass keeps one history per trajectory: where the reference
         steps the reference latents jointly with the main latents only on a prefix of the steps (inject_selfattn = 0,
         0 < inject_background < 1, :831-846) and then steps the main latents alone, the main latents keep their own
         history here instead of continuing a batch-2 one. UniPC's corrector restarts from its own last corrected
         sample, so colour guidance and background injection reach its next update only through the x0 prediction of
         the next step, as in the reference with UniPC assigned to its scheduler.
+        With HeunDiscreteScheduler each iteration is one stage of Heun's method (2N - 1 UNet evaluations for N steps);
+        each trajectory keeps the latents and prediction of its last first stage, so colour guidance and background
+        injection after a first stage reach the second stage only through its prediction, as in the reference. Where
+        the reference stops stepping the reference latents right after a first stage (inject_selfattn = 0), it would
+        add a batch-1 prediction to a batch-2 saved state; here the reference latents keep their first-stage value.
+        `callback` is called by the reference's rule (:874-877): after the second stages and the last iteration.
         With EulerAncestralDiscreteScheduler the noise z of each step is drawn as diffusers' randn_tensor draws it, fp16,
         from `generator` when one is given (on its device: a CPU generator draws on the CPU), otherwise from the global
         RNG of the sampling device. The plain pass draws [1, ...] per step, as the reference does. The rich-text pass
@@ -283,7 +292,12 @@ class RegionDiffusionXL:
         sees the latents unscaled and the blend kernel takes the step_coeffs(i) update; UniPC likewise, with
         unipc_coeffs(i) and three histories (ops.UniPCHistory). Euler Ancestral: the UNet input
         is scaled as for Euler and the blend kernel adds s_up z, z [1, ...] drawn from `generator` after the UNet pass,
-        as the reference's step draws it (:908)."""
+        as the reference's step draws it (:908). Heun: iteration i scales the UNet input by sigma_i (sigma_at(i)) and
+        the blend kernel takes the heun_coeffs(i) update; a first stage keeps the latents it stepped and the stepped
+        prediction (two fp16 tensors, referenced until the second stage reads them: the blend writes fresh outputs and
+        nothing here writes in place). The callback follows the reference's rule (:874-877): iteration i calls it when
+        (i is the last iteration or (i + 1) % scheduler.order == 0) and i % callback_steps == 0 — every iteration
+        i % callback_steps == 0 for the order-1 schedulers, only second stages and the last iteration for Heun."""
         phi = _rescale_phi(guidance_scale, guidance_rescale)
         ctx2 = torch.cat([ctx[:1], ctx[-1:]])
         pooled2 = torch.cat([pooled[:1], pooled[-1:]])
@@ -293,11 +307,13 @@ class RegionDiffusionXL:
         multistep = kind == "multistep"
         d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=latents.device) if multistep else None
         up_hist = ops.UniPCHistory(latents.numel(), latents.device) if kind == "unipc" else None
+        heun = kind == "heun"
+        xs = ds = None   # Heun: the latents and the prediction of the last first stage
         for i, t in enumerate(timesteps):
             if multistep or up_hist is not None:
                 x = latents.expand(2, -1, -1, -1)
             else:
-                sigma = self.scheduler.sigma(t)
+                sigma = self.scheduler.sigma_at(i) if heun else self.scheduler.sigma(t)
                 x = (latents / math.sqrt(sigma * sigma + 1.0)).expand(2, -1, -1, -1)
             ctrl = RegionControl(capture=self._capture, capture_row=1, kv_cache=kv)
             eps = self.unet(x, t, ctx2, {"text_embeds": pooled2, "time_ids": time_ids}, ctrl)["sample"]
@@ -319,13 +335,25 @@ class RegionDiffusionXL:
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(), guidance_rescale=phi,
                                                   step=ops.AncestralStep(dt, s_up, z))
+            elif heun:
+                lat = latents.contiguous()
+                e16, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                    latents=lat, guidance_rescale=phi,
+                                                    step=ops.HeunStep(self.scheduler.heun_coeffs(i), xs, ds))
+                if self.scheduler.is_first_stage(i):
+                    xs, ds = lat, e16
             else:
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
                                                   guidance_rescale=phi)
-            if callback is not None and i % callback_steps == 0:
+            if callback is not None and self._calls_back(i, len(timesteps), callback_steps):
                 callback(i, t, latents)
         return latents
+
+    def _calls_back(self, i, n_iterations, callback_steps):
+        """The reference's callback rule (:874-877 and :910-914; num_warmup_steps = len(timesteps) - N * order is
+        never positive here)."""
+        return (i == n_iterations - 1 or (i + 1) % self.scheduler.order == 0) and i % callback_steps == 0
 
     def build_pass_batch(self, n_regions, inject):
         """Order of the batched passes of one step and the context row each one uses.
@@ -385,6 +413,9 @@ class RegionDiffusionXL:
         # UniPC: one state of three fp32 buffers per trajectory
         st.up_hist = ops.UniPCHistory(n, dev) if st.unipc else None
         st.up_hist_ref = ops.UniPCHistory(n, dev) if st.unipc and inject else None
+        # Heun: (latents, prediction) of the last first stage per trajectory, fp16, referenced until the second stage
+        st.heun = kind == "heun"
+        st.heun_main = st.heun_ref = (None, None)
         return st
 
     def _unet_pass(self, st, x, t, local, feat_inject_step):
@@ -482,7 +513,7 @@ class RegionDiffusionXL:
         if st.multistep or st.unipc:   # scale_model_input is the identity
             scale = None
         else:
-            sigma = self.scheduler.sigma(t)
+            sigma = self.scheduler.sigma_at(i) if st.heun else self.scheduler.sigma(t)
             scale = 1.0 / math.sqrt(sigma * sigma + 1.0)                                # :784
         if feat_inject_step and st.inject:
             self._remote_qk(st, st.latents)   # collective on first use: every rank of the group, also those without passes
@@ -526,6 +557,20 @@ class RegionDiffusionXL:
             z_ref = z[1:2] if step_ref else None
             step = ops.AncestralStep(a_dt, s_up, z[0:1], z_ref)
             step_main, step_refl = ops.AncestralStep(a_dt, s_up, z[0:1]), ops.AncestralStep(a_dt, s_up, z_ref)
+        elif st.heun:
+            # each trajectory steps from its own saved state; a first stage saves the latents it steps and their
+            # prediction (on the fused exchange the reference trajectory's is written into eps_ref)
+            dt = 0.0
+            c = self.scheduler.heun_coeffs(i)
+            first = self.scheduler.is_first_stage(i)
+            st.latents = lat_in = st.latents.contiguous()
+            if step_ref:
+                st.latents_ref = ref_in = st.latents_ref.contiguous()
+            xs_ref, ds_ref = st.heun_ref if step_ref else (None, None)
+            fused = plan.world > 1 and self.fused_exchange
+            eps_ref = torch.empty_like(ref_in) if first and step_ref and fused else None
+            step = ops.HeunStep(c, *st.heun_main, xs_ref, ds_ref, eps_ref)
+            step_main, step_refl = ops.HeunStep(c, *st.heun_main), ops.HeunStep(c, xs_ref, ds_ref)
         else:
             dt = self.scheduler.dt(t)
             step = step_main = step_refl = None
@@ -559,14 +604,20 @@ class RegionDiffusionXL:
                                                               guidance_rescale=st.guidance_rescale,
                                                               step=step_main)  # :810-830
             if step_ref:
-                _, st.latents_ref = ops.region_blend_cfg(one("C"), [one("D")], st.ones, st.guidance_scale,
-                                                         latents=st.latents_ref.contiguous(), dt_sigma=dt,
-                                                         guidance_rescale=st.guidance_rescale,
-                                                         step=step_refl)
+                eps_cd, st.latents_ref = ops.region_blend_cfg(one("C"), [one("D")], st.ones, st.guidance_scale,
+                                                              latents=st.latents_ref.contiguous(), dt_sigma=dt,
+                                                              guidance_rescale=st.guidance_rescale,
+                                                              step=step_refl)
+                if st.heun:
+                    eps_ref = eps_cd
         if st.unipc:   # this step's x0 prediction becomes m1 of the next step
             st.up_hist.rotate()
             if step_ref:
                 st.up_hist_ref.rotate()
+        if st.heun and first:
+            st.heun_main = (lat_in, st.noise_pred)
+            if step_ref:
+                st.heun_ref = (ref_in, eps_ref)
         if pe is not None:
             ev[2].record()
         if st.use_guidance and float(t) < st.tfd["guidance_start_step"]:                                  # :849
@@ -588,7 +639,7 @@ class RegionDiffusionXL:
                                     inject_selfattn, inject_background, tfd, guidance_rescale, generator)
         for i, t in enumerate(timesteps):
             self.rich_text_step(st, i)
-            if callback is not None and i % callback_steps == 0:
+            if callback is not None and self._calls_back(i, len(timesteps), callback_steps):
                 callback(i, t, st.latents)
         for ex in self._exchanges.values():
             ex.check()

@@ -11,7 +11,8 @@ DDIMScheduler and DPMSolverMultistepScheduler (below) are the schedulers a diffu
 the per-step coefficients of `step_coeffs(i)`. EulerAncestralDiscreteScheduler ("Euler a", SDXL) adds fresh noise on
 every step; the SDXL sampler runs it through the fused blend kernels with `ancestral_coeffs(i)`.
 UniPCMultistepScheduler (bh2, order 2, the few-step sampler) runs through the fused blend kernels of both samplers
-with `unipc_coeffs(i)`.
+with `unipc_coeffs(i)`. HeunDiscreteScheduler (Heun's second-order method on Euler's sigma grid, two UNet evaluations
+per step) runs through the fused blend kernels of the SDXL sampler with `heun_coeffs(k)`.
 """
 import math
 from typing import NamedTuple
@@ -489,4 +490,106 @@ class EulerAncestralDiscreteScheduler(_Configured):
         dt, s_up = self.ancestral_coeffs(self.index_of(timestep))
         z = self.noise(model_output.shape, generator, model_output.device, model_output.dtype)
         prev = (sample.float() + model_output.float() * dt + z.float() * s_up).to(sample.dtype)
+        return {"prev_sample": prev} if return_dict else (prev,)
+
+
+# ---------------------------------------------------------------------------------------------------- Heun
+class HeunDiscreteScheduler(_Configured):
+    """Heun's method (Karras et al., EDM, Algorithm 1 without churn), epsilon prediction, with the SDXL config
+    (scaled-linear betas 0.00085-0.012, `leading` spacing, steps_offset=1), restating diffusers 0.18.2
+    (`schedulers/scheduling_heun_discrete.py`). PARITY UNPINNED: that source is not available here; the conventions
+    below are the definition.
+      From Euler's grid for N steps, t_0..t_{N-1} and s_0..s_{N-1}, 0 (EulerDiscreteScheduler.set_timesteps):
+        timesteps   = [t_0, t_1, t_1, ..., t_{N-1}, t_{N-1}]      2N - 1 loop iterations
+        sigmas_host = [s_0, s_1, s_1, ..., s_{N-1}, s_{N-1}, 0]   2N entries
+      num_inference_steps = N, order = 2; init_noise_sigma = sqrt(s_max^2 + 1), Euler's (the value of `leading`
+      spacing, also unpinned); alphas_cumprod: Euler's.
+      Iteration k, sigma_k = sigmas_host[k] (indexed by k: the timestep values repeat); the UNet sees
+      x / sqrt(sigma_k^2 + 1).
+        k even, first stage:  x' = x + (sigma_{k+1} - sigma_k) eps;  keeps xs = x, ds = eps, dt = sigma_{k+1} - sigma_k
+        k odd, second stage:  x' = xs + dt/2 (ds + eps)
+      The last iteration, k = 2N - 2, is a first stage to sigma = 0 (a plain Euler step); its saved state is never used.
+    The second stage restarts from xs, so the current latents reach it only through eps: whatever a sampling loop does
+    to the latents between the two stages (colour guidance, background injection) is overwritten, as in diffusers. The
+    samplers run it through the fused blend kernels with the coefficients of `heun_coeffs(k)` and the fp16 xs and ds of
+    each trajectory (ops.HeunStep); `step` is the stateful torch form in diffusers' calling convention."""
+    order = 2
+    _defaults = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                     trained_betas=None, prediction_type="epsilon", use_karras_sigmas=False,
+                     timestep_spacing="leading", steps_offset=1)
+    _unsupported = dict(trained_betas=None, prediction_type="epsilon", use_karras_sigmas=False,
+                        timestep_spacing="leading")
+
+    def __init__(self, **kw):
+        cfg = self._configure(kw)
+        self._grid = EulerDiscreteScheduler(cfg["beta_start"], cfg["beta_end"], int(cfg["num_train_timesteps"]),
+                                            int(cfg["steps_offset"]))
+        self.num_train_timesteps = self._grid.num_train_timesteps
+        self.alphas_cumprod = self._grid.alphas_cumprod
+        self.num_inference_steps = None
+        self.timesteps_host, self.sigmas_host = self._grid.timesteps_host, self._grid.sigmas_host
+        self.timesteps = self._grid.timesteps
+        self._reset()
+
+    def _reset(self):
+        self._k, self._xs, self._ds, self._dt = 0, None, None, None
+
+    @property
+    def init_noise_sigma(self):
+        return self._grid.init_noise_sigma
+
+    def set_timesteps(self, num_inference_steps, device=None):
+        g = self._grid
+        g.set_timesteps(num_inference_steps, device)
+        self.num_inference_steps = num_inference_steps
+        self.timesteps_host = np.concatenate([g.timesteps_host[:1], np.repeat(g.timesteps_host[1:], 2)])
+        self.sigmas_host = np.concatenate([g.sigmas_host[:1], np.repeat(g.sigmas_host[1:-1], 2),
+                                           g.sigmas_host[-1:]]).astype(np.float32)
+        self.timesteps = torch.from_numpy(self.timesteps_host.copy())   # host tensor, as Euler's
+        self._reset()
+
+    @staticmethod
+    def is_first_stage(k):
+        return k % 2 == 0
+
+    @property
+    def state_in_first_order(self):
+        """Whether the next `step` call is a first stage (diffusers' name)."""
+        return self._dt is None
+
+    def sigma_at(self, k):
+        return float(self.sigmas_host[k])
+
+    def scale_model_input(self, sample, timestep):
+        """x / sqrt(sigma^2 + 1) at the iteration the next `step` call makes."""
+        s = self.sigma_at(self._k)
+        return sample / ((s * s + 1.0) ** 0.5)
+
+    def heun_coeffs(self, k):
+        """(cx, ce, cs, cd) of iteration k in float64: x' = cx x + ce eps + cs xs + cd ds; (1, dt, 0, 0) at a first
+        stage, (0, dt/2, 1, dt/2) at a second, dt = sigma_{k+1} - sigma_k of the first stage."""
+        if self.is_first_stage(k):
+            return 1.0, float(self.sigmas_host[k + 1]) - float(self.sigmas_host[k]), 0.0, 0.0
+        dt = float(self.sigmas_host[k]) - float(self.sigmas_host[k - 1])
+        return 0.0, 0.5 * dt, 1.0, 0.5 * dt
+
+    def step(self, model_output, timestep, sample, return_dict=True, **kw):
+        """Stateful torch form of heun_coeffs in diffusers' calling convention (the samplers use the fused kernels
+        instead): the stage follows from the calls made since set_timesteps, as diffusers' state_in_first_order, and
+        `timestep` must be the loop's timestep of that call. Evaluated in the precision of `sample` and at least fp32."""
+        k = self._k
+        if float(timestep) != float(self.timesteps_host[k]):
+            raise ValueError(f"HeunDiscreteScheduler.step: timestep {float(timestep)} is not that of iteration {k} "
+                             f"({float(self.timesteps_host[k])})")
+        cx, ce, cs, cd = self.heun_coeffs(k)
+        dtype = torch.promote_types(sample.dtype, torch.float32)
+        x, e = sample.to(dtype), model_output.to(dtype)
+        if self.is_first_stage(k):
+            prev = cx * x + ce * e
+            self._xs, self._ds, self._dt = x, e, 2.0 * ce
+        else:
+            prev = self._xs + ce * (self._ds + e)
+            self._xs = self._ds = self._dt = None
+        self._k = k + 1
+        prev = prev.to(sample.dtype)
         return {"prev_sample": prev} if return_dict else (prev,)
