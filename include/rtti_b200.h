@@ -217,6 +217,26 @@ int rtti_region_blend_cfg_rescale_heun(const void* eps_uncond, const void* const
                                        void* latents_out, float cx, float ce, float cs, float cd, const void* xs,
                                        const void* ds, float guidance_rescale, void* stream);
 
+/* LMS forms ("_lms") of the blend entry points, for k-LMS, the fourth-order linear multistep method on Euler's sigma
+ * grid (rich-text-to-image_b200/schedulers.py, LMSDiscreteScheduler.lms_coeffs). They replace the scheduler step of
+ * models/region_diffusion_sdxl.py:837-846 and :908 with an LMSDiscreteScheduler assigned to the reference's scheduler.
+ * The blend, CFG and rescale arithmetic is that of the Euler form; the update of the latents is, in fp32,
+ *   x' = x + c0 * eps + c1 * d1 + c2 * d2 + c3 * d3      (x' rounded to fp16)
+ * with x the fp16 latents, eps the fp16-rounded (rescaled) noise prediction written to eps_out, and d1[n], d2[n], d3[n]
+ * the fp16 eps_out of the trajectory's last three steps, newest first. The terms are added in that order. d_k is read
+ * only when c_k != 0; with (c0, 0, 0, 0) the result equals the Euler form's with dt_sigma = c0, bit for bit. latents and
+ * latents_out are required; d_k is required when c_k != 0, and each is 16-byte aligned when given. The histories are
+ * only read: they must not overlap eps_out or latents_out. The other checks are those of the Euler form; on any error
+ * nothing is launched. */
+int rtti_region_blend_cfg_lms(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions,
+                              long long n, float guidance, void* eps_out, const void* latents, void* latents_out,
+                              float c0, float c1, float c2, float c3, const void* d1, const void* d2, const void* d3,
+                              void* stream);
+int rtti_region_blend_cfg_rescale_lms(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                      int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                      void* latents_out, float c0, float c1, float c2, float c3, const void* d1,
+                                      const void* d2, const void* d3, float guidance_rescale, void* stream);
+
 /* Colour-guidance loss forward + analytic backward w.r.t. the VAE decoder output.
  * Replaces models/region_diffusion_sdxl.py:857-865 (clamp, masked mean RGB, MSE*100, autograd of those).
  *   decoded [3, hw] fp32 (VAE output before /2+0.5), masks [n_colors, hw] fp32 (channel 0 of
@@ -379,6 +399,28 @@ int rtti_gather_blend_step_rescale_heun(const void* const* peer_slots, void* con
                                         float ce, float cs, float cd, const void* xs, const void* ds,
                                         const void* xs_ref, const void* ds_ref, void* eps_ref_out,
                                         unsigned int step_id, float guidance_rescale, void* stream);
+
+/* LMS forms of rtti_gather_blend_step / rtti_gather_blend_step_rescale (the update of rtti_region_blend_cfg_lms; they
+ * replace models/region_diffusion_sdxl.py:837-846 with an LMSDiscreteScheduler assigned to the reference's scheduler).
+ * The reference-latent trajectory, when latents_ref is given, is stepped with the same coefficients on its own history
+ * d1_ref / d2_ref / d3_ref (with the requirements of d1 / d2 / d3). eps_ref_out[n], optional (null: not written; given
+ * without latents_ref: RTTI_ERR_ARG; 16-byte aligned), receives that trajectory's fp16-rounded (rescaled) noise
+ * prediction, the eps_out of the single-GPU form called on the C/D pair with one region and a mask of ones: the newest
+ * entry of its history for the next step. For the same noise predictions the outputs equal those of the single-GPU
+ * forms bit for bit, whatever the world size. Same protocol and slot layout as the Euler forms. */
+int rtti_gather_blend_step_lms(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                               const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                               float guidance, void* eps_out, const void* latents, void* latents_out,
+                               const void* latents_ref, void* latents_ref_out, float c0, float c1, float c2, float c3,
+                               const void* d1, const void* d2, const void* d3, const void* d1_ref, const void* d2_ref,
+                               const void* d3_ref, void* eps_ref_out, unsigned int step_id, void* stream);
+int rtti_gather_blend_step_rescale_lms(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                       const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                       long long n, float guidance, void* eps_out, const void* latents,
+                                       void* latents_out, const void* latents_ref, void* latents_ref_out, float c0,
+                                       float c1, float c2, float c3, const void* d1, const void* d2, const void* d3,
+                                       const void* d1_ref, const void* d2_ref, const void* d3_ref, void* eps_ref_out,
+                                       unsigned int step_id, float guidance_rescale, void* stream);
 
 /* Stripe-parallel colour guidance (multi-GPU; new relative to the single-GPU reference, which back-propagates
  * through the batch-1 VAE decoder on one device: models/region_diffusion_sdxl.py:849-867). Every activation of

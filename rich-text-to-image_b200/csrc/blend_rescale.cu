@@ -78,8 +78,15 @@ struct RescaleHeunParams : RescaleParams {
   __half* eps_ref_out;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun update of the main (REF
-// false) / reference (REF true) trajectory
+// the LMS form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory, and where the
+// reference trajectory's rescaled fp16 prediction goes (gather form only; null: not written)
+struct RescaleLmsParams : RescaleParams {
+  LmsStep ls, ls_ref;
+  __half* eps_ref_out;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun / LMS update of the main
+// (REF false) / reference (REF true) trajectory
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleParams& p, long long, const float* e16, float* x) {
 #pragma unroll
@@ -101,10 +108,16 @@ template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleHeunParams& p, long long v, const float* e16, float* x) {
   heun_step8(REF ? p.hs_ref : p.hs, v, e16, x);
 }
+template <bool REF>
+__device__ __forceinline__ void rs_step(const RescaleLmsParams& p, long long v, const float* e16, float* x) {
+  lms_step8(REF ? p.ls_ref : p.ls, v, e16, x);
+}
 
-// the output of the reference trajectory's prediction: only the Heun form stores it (the ds of its first stage)
+// the output of the reference trajectory's prediction: only the Heun form (the ds of its first stage) and the LMS form
+// (the newest entry of its history) store it
 __device__ __forceinline__ __half* rs_ref_eps(const RescaleParams&) { return nullptr; }
 __device__ __forceinline__ __half* rs_ref_eps(const RescaleHeunParams& p) { return p.eps_ref_out; }
+__device__ __forceinline__ __half* rs_ref_eps(const RescaleLmsParams& p) { return p.eps_ref_out; }
 
 // (count, mean, m2) of eps_text and of eps_cfg over the same elements
 struct PairStats { int n; float mt, qt, mc, qc; };
@@ -316,6 +329,14 @@ __global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
   blend_rescale_body<PEER>(p, cfg_s, sm);
 }
 
+template <bool PEER>
+__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
+    blend_rescale_lms_kernel(const __grid_constant__ RescaleLmsParams p) {
+  extern __shared__ float4 cfg_s[];
+  __shared__ RescaleSmem sm;
+  blend_rescale_body<PEER>(p, cfg_s, sm);
+}
+
 // the kernel of each parameter type
 template <bool PEER>
 const void* rescale_kernel(const RescaleParams&) { return (const void*)blend_rescale_kernel<PEER>; }
@@ -327,6 +348,8 @@ template <bool PEER>
 const void* rescale_kernel(const RescaleUniPCParams&) { return (const void*)blend_rescale_unipc_kernel<PEER>; }
 template <bool PEER>
 const void* rescale_kernel(const RescaleHeunParams&) { return (const void*)blend_rescale_heun_kernel<PEER>; }
+template <bool PEER>
+const void* rescale_kernel(const RescaleLmsParams&) { return (const void*)blend_rescale_lms_kernel<PEER>; }
 
 // threads per CTA and vectors per thread: a function of n only
 void rescale_plan(long long n, int& threads, int& vpt) {
@@ -354,6 +377,8 @@ int launch_rescale(P& p, void* stream) {
     blend_rescale_unipc_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else if constexpr (std::is_same<P, RescaleHeunParams>::value)
     blend_rescale_heun_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
+  else if constexpr (std::is_same<P, RescaleLmsParams>::value)
+    blend_rescale_lms_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else
     blend_rescale_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
@@ -586,6 +611,45 @@ extern "C" int rtti_gather_blend_step_rescale_heun(const void* const* peer_slots
   p.phi = guidance_rescale;
   p.hs = HeunStep{cx, ce, cs, cd, (const __half*)xs, (const __half*)ds};
   p.hs_ref = HeunStep{cx, ce, cs, cd, (const __half*)xs_ref, (const __half*)ds_ref};
+  p.eps_ref_out = (__half*)eps_ref_out;
+  return launch_rescale<true>(p, stream);
+}
+
+extern "C" int rtti_region_blend_cfg_rescale_lms(const void* eps_uncond, const void* const* eps_region,
+                                                 const float* masks, int n_regions, long long n, float guidance,
+                                                 void* eps_out, const void* latents, void* latents_out, float c0,
+                                                 float c1, float c2, float c3, const void* d1, const void* d2,
+                                                 const void* d3, float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleLmsParams p{};
+  int rc = rescale_args(eps_uncond, eps_region, masks, n_regions, n, guidance, eps_out, latents, latents_out, p);
+  if (rc == RTTI_OK) rc = lms_step_args(c1, c2, c3, d1, d2, d3);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.ls = LmsStep{c0, c1, c2, c3, (const __half*)d1, (const __half*)d2, (const __half*)d3};
+  return launch_rescale<false>(p, stream);
+}
+
+extern "C" int rtti_gather_blend_step_rescale_lms(const void* const* peer_slots, void* const* peer_flags, int world,
+                                                  int rank, const int* slot_owner, int n_slots, int n_regions,
+                                                  const float* masks, long long n, float guidance, void* eps_out,
+                                                  const void* latents, void* latents_out, const void* latents_ref,
+                                                  void* latents_ref_out, float c0, float c1, float c2, float c3,
+                                                  const void* d1, const void* d2, const void* d3, const void* d1_ref,
+                                                  const void* d2_ref, const void* d3_ref, void* eps_ref_out,
+                                                  unsigned int step_id, float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  if (eps_ref_out != nullptr && latents_ref == nullptr) return RTTI_ERR_ARG;
+  RescaleLmsParams p{};
+  int rc = gather_rescale_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                               eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = lms_step_args(c1, c2, c3, d1, d2, d3);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = lms_step_args(c1, c2, c3, d1_ref, d2_ref, d3_ref);
+  if (rc == RTTI_OK && ((uintptr_t)eps_ref_out & 15)) rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.ls = LmsStep{c0, c1, c2, c3, (const __half*)d1, (const __half*)d2, (const __half*)d3};
+  p.ls_ref = LmsStep{c0, c1, c2, c3, (const __half*)d1_ref, (const __half*)d2_ref, (const __half*)d3_ref};
   p.eps_ref_out = (__half*)eps_ref_out;
   return launch_rescale<true>(p, stream);
 }

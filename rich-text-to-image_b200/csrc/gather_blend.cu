@@ -81,8 +81,15 @@ struct GatherBlendHeunParams : GatherBlendParams {
   __half* eps_ref_out;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun update of the main /
-// reference trajectory
+// the LMS form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory, and where the
+// reference trajectory's fp16 prediction goes (null: not written)
+struct GatherBlendLmsParams : GatherBlendParams {
+  LmsStep ls, ls_ref;
+  __half* eps_ref_out;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun / LMS update of the
+// main / reference trajectory
 __device__ __forceinline__ void gb_step(const GatherBlendParams& p, bool, long long, const float* e16, float* x) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
@@ -100,10 +107,17 @@ __device__ __forceinline__ void gb_step(const GatherBlendUniPCParams& p, bool re
 __device__ __forceinline__ void gb_step(const GatherBlendHeunParams& p, bool ref, long long v, const float* e16, float* x) {
   heun_step8(ref ? p.hs_ref : p.hs, v, e16, x);
 }
+__device__ __forceinline__ void gb_step(const GatherBlendLmsParams& p, bool ref, long long v, const float* e16, float* x) {
+  lms_step8(ref ? p.ls_ref : p.ls, v, e16, x);
+}
 
-// the reference trajectory's fp16 prediction: only the Heun form stores it (the ds of its first stage)
+// the reference trajectory's fp16 prediction: only the Heun form (the ds of its first stage) and the LMS form (the
+// newest entry of its history) store it
 __device__ __forceinline__ void gb_ref_eps(const GatherBlendParams&, long long, const H8&) {}
 __device__ __forceinline__ void gb_ref_eps(const GatherBlendHeunParams& p, long long v8, const H8& h) {
+  if (p.eps_ref_out != nullptr) *reinterpret_cast<H8*>(p.eps_ref_out + v8 * 8) = h;
+}
+__device__ __forceinline__ void gb_ref_eps(const GatherBlendLmsParams& p, long long v8, const H8& h) {
   if (p.eps_ref_out != nullptr) *reinterpret_cast<H8*>(p.eps_ref_out + v8 * 8) = h;
 }
 
@@ -194,6 +208,10 @@ __global__ void __launch_bounds__(128) gather_blend_unipc_kernel(const GatherBle
   gather_blend_body(p);
 }
 __global__ void __launch_bounds__(128) gather_blend_heun_kernel(const GatherBlendHeunParams p) {
+  GB_PUBLISH_AND_WAIT(p);
+  gather_blend_body(p);
+}
+__global__ void __launch_bounds__(128) gather_blend_lms_kernel(const GatherBlendLmsParams p) {
   GB_PUBLISH_AND_WAIT(p);
   gather_blend_body(p);
 }
@@ -344,5 +362,31 @@ extern "C" int rtti_gather_blend_step_heun(const void* const* peer_slots, void* 
   p.eps_ref_out = (__half*)eps_ref_out;
   const long long nv = n / 8;
   gather_blend_heun_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+extern "C" int rtti_gather_blend_step_lms(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                          const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                          long long n, float guidance, void* eps_out, const void* latents,
+                                          void* latents_out, const void* latents_ref, void* latents_ref_out, float c0,
+                                          float c1, float c2, float c3, const void* d1, const void* d2, const void* d3,
+                                          const void* d1_ref, const void* d2_ref, const void* d3_ref,
+                                          void* eps_ref_out, unsigned int step_id, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  if (eps_ref_out != nullptr && latents_ref == nullptr) return RTTI_ERR_ARG;
+  GatherBlendLmsParams p{};
+  int rc = gather_blend_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                             eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = lms_step_args(c1, c2, c3, d1, d2, d3);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = lms_step_args(c1, c2, c3, d1_ref, d2_ref, d3_ref);
+  if (rc == RTTI_OK && (((uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out |
+                         (uintptr_t)latents_ref | (uintptr_t)latents_ref_out | (uintptr_t)eps_ref_out) & 15))
+    rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.ls = LmsStep{c0, c1, c2, c3, (const __half*)d1, (const __half*)d2, (const __half*)d3};
+  p.ls_ref = LmsStep{c0, c1, c2, c3, (const __half*)d1_ref, (const __half*)d2_ref, (const __half*)d3_ref};
+  p.eps_ref_out = (__half*)eps_ref_out;
+  const long long nv = n / 8;
+  gather_blend_lms_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

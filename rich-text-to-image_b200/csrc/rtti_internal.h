@@ -51,6 +51,12 @@ inline int heun_step_args(float cs, float cd, const void* xs, const void* ds) {
   return (((uintptr_t)xs | (uintptr_t)ds) & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
 }
 
+// the prediction history of an LMS blend step: d_k required when c_k != 0; each 16-byte aligned when given
+inline int lms_step_args(float c1, float c2, float c3, const void* d1, const void* d2, const void* d3) {
+  if ((c1 != 0.f && !d1) || (c2 != 0.f && !d2) || (c3 != 0.f && !d3)) return RTTI_ERR_ARG;
+  return (((uintptr_t)d1 | (uintptr_t)d2 | (uintptr_t)d3) & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
+}
+
 #ifdef __CUDACC__
 // GroupNorm statistics of a set of values as (count n, mean, m2 = sum of squared deviations from the mean), merged with
 // the pairwise update of Chan, Golub & LeVeque. Unlike a one-pass E[x^2] - E[x]^2 in fp32, which loses about
@@ -226,6 +232,41 @@ __device__ __forceinline__ void heun_step8(const HeunStep& s, long long v, const
 #pragma unroll
     for (int i = 0; i < 8; ++i) x[i] = fmaf(p[i], s.cs, x[i]);
   }
+}
+
+// The LMS update (schedulers.py, LMSDiscreteScheduler.lms_coeffs), in fp32:
+//   x' = x + c0 * eps + c1 * d1 + c2 * d2 + c3 * d3
+// with d1, d2, d3 the fp16 [n] noise predictions of the last three steps of the trajectory, newest first. d_k is read
+// (128-bit) only when c_k != 0; the history loads are all issued before the first FMA so that their latencies overlap.
+// The terms are added in the order above, the Euler update first, so (c0, 0, 0, 0) gives the Euler bits with
+// dt_sigma = c0.
+struct LmsStep {
+  float c0, c1, c2, c3;
+  const __half* d1;
+  const __half* d2;
+  const __half* d3;
+};
+
+__device__ __forceinline__ void lms_fma8(const uint4& u, float c, float* x) {
+  const __half2* h = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 t = __half22float2(h[i]);
+    x[2 * i] = fmaf(t.x, c, x[2 * i]);
+    x[2 * i + 1] = fmaf(t.y, c, x[2 * i + 1]);
+  }
+}
+
+__device__ __forceinline__ void lms_step8(const LmsStep& s, long long v, const float* e16, float* x) {
+  uint4 h1, h2, h3;
+  if (s.c1 != 0.f) h1 = *reinterpret_cast<const uint4*>(s.d1 + v * 8);
+  if (s.c2 != 0.f) h2 = *reinterpret_cast<const uint4*>(s.d2 + v * 8);
+  if (s.c3 != 0.f) h3 = *reinterpret_cast<const uint4*>(s.d3 + v * 8);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], s.c0, x[i]);
+  if (s.c1 != 0.f) lms_fma8(h1, s.c1, x);
+  if (s.c2 != 0.f) lms_fma8(h2, s.c2, x);
+  if (s.c3 != 0.f) lms_fma8(h3, s.c3, x);
 }
 
 // fixed-order tree over the 32 lanes of a warp; lane 0 ends with the statistics of every lane

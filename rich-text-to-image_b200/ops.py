@@ -354,6 +354,52 @@ class HeunStep:
         return a + ([_ptr(self.xs_ref), _ptr(self.ds_ref), _ptr(self.eps_ref_out)] if ref else [])
 
 
+def _overlap(a, b):
+    """Whether the storage spans of two tensors intersect."""
+    a0, b0 = a.data_ptr(), b.data_ptr()
+    return a0 < b0 + b.numel() * b.element_size() and b0 < a0 + a.numel() * a.element_size()
+
+
+class LMSStep:
+    """The LMS update of one blend call: `coeffs` (c0, c1, c2, c3) from schedulers.LMSDiscreteScheduler.lms_coeffs,
+    x' = x + c0 eps + c1 d1 + c2 d2 + c3 d3, with d1, d2, d3 the fp16 [n] stepped noise predictions of the trajectory's
+    last three steps, newest first (d_k read when c_k != 0; may be None otherwise). d1_ref / d2_ref / d3_ref: the
+    reference-latent trajectory's; eps_ref_out: an fp16 [n] tensor that receives that trajectory's stepped prediction,
+    or None (gather_blend_step only). The histories are only read; no output may overlap them."""
+
+    def __init__(self, coeffs, d1, d2, d3, d1_ref=None, d2_ref=None, d3_ref=None, eps_ref_out=None):
+        self.coeffs = tuple(float(c) for c in coeffs)
+        if len(self.coeffs) != 4:
+            raise _lib.RttiError(f"LMS blend: coeffs must be (c0, c1, c2, c3), got {len(self.coeffs)} values")
+        self.d, self.d_ref, self.eps_ref_out = (d1, d2, d3), (d1_ref, d2_ref, d3_ref), eps_ref_out
+
+    def _check(self, n, ref, outs=()):
+        """`outs`: the output tensors of the call, which must not overlap a history."""
+        c = self.coeffs[1:]
+        items = [(t, ck != 0.0, f"d{k + 1}") for k, (t, ck) in enumerate(zip(self.d, c))]
+        if ref:
+            items += [(t, ck != 0.0, f"d{k + 1}_ref") for k, (t, ck) in enumerate(zip(self.d_ref, c))]
+            items.append((self.eps_ref_out, False, "eps_ref_out"))
+        elif self.eps_ref_out is not None:
+            raise _lib.RttiError("LMS blend: eps_ref_out needs the reference latents")
+        for t, need, name in items:
+            if t is None:
+                if need:
+                    raise _lib.RttiError(f"LMS blend: {name} is required")
+                continue
+            _req(t, _F16, name)
+            if not t.is_contiguous() or t.numel() != n:
+                raise _lib.RttiError(f"LMS blend: {name} must be a contiguous fp16 tensor of {n} elements")
+        outs = [o for o in outs if o is not None] + ([self.eps_ref_out] if ref and self.eps_ref_out is not None else [])
+        for t, _, name in items:
+            if t is not None and name != "eps_ref_out" and any(_overlap(t, o) for o in outs):
+                raise _lib.RttiError(f"LMS blend: {name} overlaps an output of the call")
+
+    def args(self, ref=False):
+        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(t) for t in self.d]
+        return a + ([_ptr(t) for t in self.d_ref] + [_ptr(self.eps_ref_out)] if ref else [])
+
+
 def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0,
                      step=None):
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
@@ -365,7 +411,9 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     Euler Ancestral update (rtti_region_blend_cfg_anc / rtti_region_blend_cfg_rescale_anc; dt_sigma is not used); a
     UniPCStep — the UniPC update (rtti_region_blend_cfg_unipc / rtti_region_blend_cfg_rescale_unipc; dt_sigma is not
     used); a HeunStep — the Heun update (rtti_region_blend_cfg_heun / rtti_region_blend_cfg_rescale_heun; dt_sigma is
-    not used, nor are xs_ref / ds_ref; eps_ref_out must be None)."""
+    not used, nor are xs_ref / ds_ref; eps_ref_out must be None); an LMSStep — the LMS update (rtti_region_blend_cfg_lms
+    / rtti_region_blend_cfg_rescale_lms; dt_sigma is not used, nor are d1_ref / d2_ref / d3_ref; eps_ref_out must be
+    None)."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -376,7 +424,20 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    if isinstance(step, HeunStep):
+    if isinstance(step, LMSStep):
+        if latents is None:
+            raise _lib.RttiError("region_blend_cfg: an LMS step needs the latents")
+        step._check(n, False, (eps_out, lat_out))
+        if guidance_rescale == 0.0:
+            rc = lib.rtti_region_blend_cfg_lms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                               _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_lms")
+        else:
+            rc = lib.rtti_region_blend_cfg_rescale_lms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                       _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
+                                                       float(guidance_rescale), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_rescale_lms")
+    elif isinstance(step, HeunStep):
         if latents is None:
             raise _lib.RttiError("region_blend_cfg: a Heun step needs the latents")
         step._check(n, False)
@@ -514,7 +575,8 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     rtti_gather_blend_step_rescale_anc); a UniPCStep (with `ref` when latents_ref is given) — the UniPC update
     (rtti_gather_blend_step_unipc / rtti_gather_blend_step_rescale_unipc); a HeunStep (with xs_ref / ds_ref, and
     optionally eps_ref_out, when latents_ref is given) — the Heun update (rtti_gather_blend_step_heun /
-    rtti_gather_blend_step_rescale_heun).
+    rtti_gather_blend_step_rescale_heun); an LMSStep (with d1_ref / d2_ref / d3_ref, and optionally eps_ref_out, when
+    latents_ref is given) — the LMS update (rtti_gather_blend_step_lms / rtti_gather_blend_step_rescale_lms).
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
@@ -525,7 +587,17 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    if isinstance(step, HeunStep):
+    if isinstance(step, LMSStep):
+        step._check(n, latents_ref is not None, (eps, lat_out, ref_out))
+        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
+                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
+        args += step.args(ref=True) + [int(step_id)]
+        if guidance_rescale == 0.0:
+            _lib.check(lib.rtti_gather_blend_step_lms(*args, _stream()), "rtti_gather_blend_step_lms")
+        else:
+            _lib.check(lib.rtti_gather_blend_step_rescale_lms(*args, float(guidance_rescale), _stream()),
+                       "rtti_gather_blend_step_rescale_lms")
+    elif isinstance(step, HeunStep):
         step._check(n, latents_ref is not None)
         args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
                 float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]

@@ -10,8 +10,9 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
   * region blend + CFG (+ guidance rescale) + scheduler update is one kernel (rtti_region_blend_cfg, or
     rtti_region_blend_cfg_rescale with guidance_rescale > 0; their "_ms" forms for DDIM / DPM-Solver++(2M), which
     keep one fp32 history of the x0 prediction per trajectory, "_anc" forms for Euler Ancestral, which add the
-    noise drawn for the step, "_unipc" forms for UniPC, which keep three fp32 histories per trajectory, and "_heun"
-    forms for Heun's method, which read the fp16 latents and prediction saved at the first stage);
+    noise drawn for the step, "_unipc" forms for UniPC, which keep three fp32 histories per trajectory, "_heun"
+    forms for Heun's method, which read the fp16 latents and prediction saved at the first stage, and "_lms" forms for
+    k-LMS, which read the fp16 predictions of the last three steps);
     colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
@@ -26,7 +27,7 @@ import torch
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
 from .schedulers import (MULTISTEP_SCHEDULERS, DDIMScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
-                         HeunDiscreteScheduler, UniPCMultistepScheduler)
+                         HeunDiscreteScheduler, LMSDiscreteScheduler, UniPCMultistepScheduler)
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -39,8 +40,11 @@ def _rescale_phi(guidance_scale, guidance_rescale):
 def _step_kind(scheduler):
     """The fused update a scheduler runs as: "euler" (EulerDiscreteScheduler), "ancestral"
     (EulerAncestralDiscreteScheduler: the Euler update plus the noise term, ancestral_coeffs), "multistep"
-    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs), "unipc" (UniPCMultistepScheduler, unipc_coeffs) or
-    "heun" (HeunDiscreteScheduler, heun_coeffs). Any other scheduler has no fused update here."""
+    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs), "unipc" (UniPCMultistepScheduler, unipc_coeffs),
+    "heun" (HeunDiscreteScheduler, heun_coeffs) or "lms" (LMSDiscreteScheduler, lms_coeffs). Any other scheduler has no
+    fused update here."""
+    if isinstance(scheduler, LMSDiscreteScheduler):
+        return "lms"
     if isinstance(scheduler, HeunDiscreteScheduler):
         return "heun"
     if isinstance(scheduler, UniPCMultistepScheduler):
@@ -53,7 +57,7 @@ def _step_kind(scheduler):
         return "multistep"
     raise TypeError(f"RegionDiffusionXL: unsupported scheduler {type(scheduler).__name__}; supported: "
                     "EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler, "
-                    "UniPCMultistepScheduler, HeunDiscreteScheduler (rtti_b200.schedulers)")
+                    "UniPCMultistepScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler (rtti_b200.schedulers)")
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -219,8 +223,9 @@ class RegionDiffusionXL:
         guidance_scale > 1) rescales the CFG prediction as diffusers' rescale_noise_cfg in both passes; the reference
         implements it for the plain pass only (:903-905) and raises NotImplementedError in the rich-text pass (:827-830).
         `self.scheduler` may be EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler,
-        DPMSolverMultistepScheduler, UniPCMultistepScheduler or HeunDiscreteScheduler (schedulers.py); `eta` > 0
-        (stochastic DDIM, which the reference's plain pass forwards to DDIM) is not implemented.
+        DPMSolverMultistepScheduler, UniPCMultistepScheduler, HeunDiscreteScheduler or LMSDiscreteScheduler
+        (schedulers.py); `eta` > 0 (stochastic DDIM, which the reference's plain pass forwards to DDIM) is not
+        implemented.
         With a multistep or UniPC scheduler the rich-text pass keeps one history per trajectory: where the reference
         steps the reference latents jointly with the main latents only on a prefix of the steps (inject_selfattn = 0,
         0 < inject_background < 1, :831-846) and then steps the main latents alone, the main latents keep their own
@@ -233,6 +238,11 @@ class RegionDiffusionXL:
         the reference stops stepping the reference latents right after a first stage (inject_selfattn = 0), it would
         add a batch-1 prediction to a batch-2 saved state; here the reference latents keep their first-stage value.
         `callback` is called by the reference's rule (:874-877): after the second stages and the last iteration.
+        With LMSDiscreteScheduler each trajectory keeps the fp16 predictions of its last three steps. Every step starts
+        from the current latents, so colour guidance and background injection carry into the next update in full. As
+        with the multistep schedulers, where the reference steps the reference latents jointly only on a prefix of the
+        steps (inject_selfattn = 0, 0 < inject_background < 1), it would go on to add a batch-1 prediction to batch-2
+        ones; here each trajectory keeps its own history.
         With EulerAncestralDiscreteScheduler the noise z of each step is drawn as diffusers' randn_tensor draws it, fp16,
         from `generator` when one is given (on its device: a CPU generator draws on the CPU), otherwise from the global
         RNG of the sampling device. The plain pass draws [1, ...] per step, as the reference does. The rich-text pass
@@ -297,7 +307,10 @@ class RegionDiffusionXL:
         prediction (two fp16 tensors, referenced until the second stage reads them: the blend writes fresh outputs and
         nothing here writes in place). The callback follows the reference's rule (:874-877): iteration i calls it when
         (i is the last iteration or (i + 1) % scheduler.order == 0) and i % callback_steps == 0 — every iteration
-        i % callback_steps == 0 for the order-1 schedulers, only second stages and the last iteration for Heun."""
+        i % callback_steps == 0 for the order-1 schedulers, only second stages and the last iteration for Heun.
+        LMS: the UNet input is scaled as for Euler and the blend kernel takes the lms_coeffs(i) update on the fp16
+        predictions of the last three steps (blend outputs, referenced while they are in the history; nothing writes
+        them in place)."""
         phi = _rescale_phi(guidance_scale, guidance_rescale)
         ctx2 = torch.cat([ctx[:1], ctx[-1:]])
         pooled2 = torch.cat([pooled[:1], pooled[-1:]])
@@ -309,6 +322,7 @@ class RegionDiffusionXL:
         up_hist = ops.UniPCHistory(latents.numel(), latents.device) if kind == "unipc" else None
         heun = kind == "heun"
         xs = ds = None   # Heun: the latents and the prediction of the last first stage
+        lms_hist = (None, None, None)   # LMS: the predictions of the last three steps, newest first
         for i, t in enumerate(timesteps):
             if multistep or up_hist is not None:
                 x = latents.expand(2, -1, -1, -1)
@@ -342,6 +356,11 @@ class RegionDiffusionXL:
                                                     step=ops.HeunStep(self.scheduler.heun_coeffs(i), xs, ds))
                 if self.scheduler.is_first_stage(i):
                     xs, ds = lat, e16
+            elif kind == "lms":
+                e16, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                    latents=latents.contiguous(), guidance_rescale=phi,
+                                                    step=ops.LMSStep(self.scheduler.lms_coeffs(i), *lms_hist))
+                lms_hist = (e16,) + lms_hist[:2]
             else:
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
@@ -416,6 +435,9 @@ class RegionDiffusionXL:
         # Heun: (latents, prediction) of the last first stage per trajectory, fp16, referenced until the second stage
         st.heun = kind == "heun"
         st.heun_main = st.heun_ref = (None, None)
+        # LMS: the fp16 predictions of the last three steps per trajectory, newest first
+        st.lms = kind == "lms"
+        st.lms_main = st.lms_ref = (None, None, None)
         return st
 
     def _unet_pass(self, st, x, t, local, feat_inject_step):
@@ -571,6 +593,16 @@ class RegionDiffusionXL:
             eps_ref = torch.empty_like(ref_in) if first and step_ref and fused else None
             step = ops.HeunStep(c, *st.heun_main, xs_ref, ds_ref, eps_ref)
             step_main, step_refl = ops.HeunStep(c, *st.heun_main), ops.HeunStep(c, xs_ref, ds_ref)
+        elif st.lms:
+            # each trajectory steps on its own history (on the fused exchange the reference trajectory's prediction is
+            # written into eps_ref)
+            dt = 0.0
+            c = self.scheduler.lms_coeffs(i)
+            hist_ref = st.lms_ref if step_ref else (None, None, None)
+            fused = plan.world > 1 and self.fused_exchange
+            eps_ref = torch.empty_like(st.latents_ref) if step_ref and fused else None
+            step = ops.LMSStep(c, *st.lms_main, *hist_ref, eps_ref)
+            step_main, step_refl = ops.LMSStep(c, *st.lms_main), ops.LMSStep(c, *hist_ref)
         else:
             dt = self.scheduler.dt(t)
             step = step_main = step_refl = None
@@ -608,7 +640,7 @@ class RegionDiffusionXL:
                                                               latents=st.latents_ref.contiguous(), dt_sigma=dt,
                                                               guidance_rescale=st.guidance_rescale,
                                                               step=step_refl)
-                if st.heun:
+                if st.heun or st.lms:
                     eps_ref = eps_cd
         if st.unipc:   # this step's x0 prediction becomes m1 of the next step
             st.up_hist.rotate()
@@ -618,6 +650,10 @@ class RegionDiffusionXL:
             st.heun_main = (lat_in, st.noise_pred)
             if step_ref:
                 st.heun_ref = (ref_in, eps_ref)
+        if st.lms:
+            st.lms_main = (st.noise_pred,) + st.lms_main[:2]
+            if step_ref:
+                st.lms_ref = (eps_ref,) + st.lms_ref[:2]
         if pe is not None:
             ev[2].record()
         if st.use_guidance and float(t) < st.tfd["guidance_start_step"]:                                  # :849

@@ -12,7 +12,9 @@ the per-step coefficients of `step_coeffs(i)`. EulerAncestralDiscreteScheduler (
 every step; the SDXL sampler runs it through the fused blend kernels with `ancestral_coeffs(i)`.
 UniPCMultistepScheduler (bh2, order 2, the few-step sampler) runs through the fused blend kernels of both samplers
 with `unipc_coeffs(i)`. HeunDiscreteScheduler (Heun's second-order method on Euler's sigma grid, two UNet evaluations
-per step) runs through the fused blend kernels of the SDXL sampler with `heun_coeffs(k)`.
+per step) runs through the fused blend kernels of the SDXL sampler with `heun_coeffs(k)`. LMSDiscreteScheduler (k-LMS,
+the fourth-order linear multistep method on Euler's sigma grid) runs through the fused blend kernels of the SDXL sampler
+with `lms_coeffs(i)`.
 """
 import math
 from typing import NamedTuple
@@ -591,5 +593,94 @@ class HeunDiscreteScheduler(_Configured):
             prev = self._xs + ce * (self._ds + e)
             self._xs = self._ds = self._dt = None
         self._k = k + 1
+        prev = prev.to(sample.dtype)
+        return {"prev_sample": prev} if return_dict else (prev,)
+
+
+# ---------------------------------------------------------------------------------------------------- LMS
+class LMSDiscreteScheduler(_Configured):
+    """k-LMS, the linear multistep method of order 4 on the probability-flow ODE dx/dsigma = eps, epsilon prediction, with
+    the SDXL config (scaled-linear betas 0.00085-0.012, `leading` spacing, steps_offset=1), restating diffusers 0.18.2
+    (`schedulers/scheduling_lms_discrete.py`, `step(order=4)`). PARITY UNPINNED: that source is not available here; the
+    conventions below are the definition.
+      timesteps, sigmas_host (s_0..s_{N-1}, 0), init_noise_sigma, scale_model_input, alphas_cumprod: those of
+      EulerDiscreteScheduler. order = 1: one UNet evaluation per step.
+      step i, with eps_i the step's prediction and p = min(i + 1, 4):
+        x' = x + sum_{k<p} c_k eps_{i-k},   c_k = integral from s_i to s_{i+1} of l_k(tau) dtau
+      where l_k is the Lagrange basis polynomial on the nodes s_i, s_{i-1}, ..., s_{i-p+1} with l_k(s_{i-k}) = 1.
+    diffusers integrates l_k with scipy.integrate.quad on a float32 integrand; `lms_coeffs` integrates it in closed form
+    in float64 from the same float32 nodes. Every step starts from the current latents, so whatever a sampling loop does
+    to the latents between steps (colour guidance, background injection) carries into the next update in full. Not a
+    subclass of EulerDiscreteScheduler: its `dt` is not this scheduler's step. The samplers run it through the fused
+    blend kernels with the coefficients of `lms_coeffs(i)` and the fp16 predictions of each trajectory's last three
+    steps (ops.LMSStep); `step` is the stateful torch form in diffusers' calling convention."""
+    order = 1
+    max_order = 4
+    _defaults = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                     trained_betas=None, prediction_type="epsilon", use_karras_sigmas=False,
+                     timestep_spacing="leading", steps_offset=1)
+    _unsupported = dict(trained_betas=None, prediction_type="epsilon", use_karras_sigmas=False,
+                        timestep_spacing="leading")
+
+    def __init__(self, **kw):
+        cfg = self._configure(kw)
+        self._grid = EulerDiscreteScheduler(cfg["beta_start"], cfg["beta_end"], int(cfg["num_train_timesteps"]),
+                                            int(cfg["steps_offset"]))
+        self.num_train_timesteps = self._grid.num_train_timesteps
+        self.alphas_cumprod = self._grid.alphas_cumprod
+        self.num_inference_steps = None
+        self._take_grid()
+
+    def _take_grid(self):
+        self.timesteps, self.timesteps_host, self.sigmas_host = \
+            self._grid.timesteps, self._grid.timesteps_host, self._grid.sigmas_host
+        self.derivatives = []
+
+    @property
+    def init_noise_sigma(self):
+        return self._grid.init_noise_sigma
+
+    def set_timesteps(self, num_inference_steps, device=None):
+        self._grid.set_timesteps(num_inference_steps, device)
+        self.num_inference_steps = num_inference_steps
+        self._take_grid()
+
+    def index_of(self, timestep):
+        return self._grid.index_of(timestep)
+
+    def sigma(self, timestep):
+        return self._grid.sigma(timestep)
+
+    def scale_model_input(self, sample, timestep):
+        return self._grid.scale_model_input(sample, timestep)
+
+    def lms_coeffs(self, i):
+        """(c0, c1, c2, c3) of step i in float64: x' = x + c0 eps_i + c1 eps_{i-1} + c2 eps_{i-2} + c3 eps_{i-3};
+        c_k = 0 for k >= min(i + 1, 4). Their sum is sigma_{i+1} - sigma_i."""
+        sig = self.sigmas_host
+        p = min(i + 1, self.max_order)
+        nodes = [float(sig[i - j]) for j in range(p)]
+        lo, hi = float(sig[i]), float(sig[i + 1])
+        out = [0.0] * self.max_order
+        for k in range(p):
+            basis = np.array([1.0])
+            for j in range(p):
+                if j != k:
+                    basis = np.polynomial.polynomial.polymul(basis, np.array([-nodes[j], 1.0]) / (nodes[k] - nodes[j]))
+            prim = np.polynomial.polynomial.polyint(basis)
+            out[k] = float(np.polynomial.polynomial.polyval(hi, prim) - np.polynomial.polynomial.polyval(lo, prim))
+        return tuple(out)
+
+    def step(self, model_output, timestep, sample, return_dict=True, **kw):
+        """Stateful torch form of lms_coeffs in diffusers' calling convention (the samplers use the fused kernels
+        instead): keeps the predictions of the last four calls since set_timesteps. Evaluated in the precision of
+        `sample` and at least fp32."""
+        i = self.index_of(timestep)
+        dtype = torch.promote_types(sample.dtype, torch.float32)
+        self.derivatives = [model_output.to(dtype)] + self.derivatives[:self.max_order - 1]
+        prev = sample.to(dtype)
+        for c, d in zip(self.lms_coeffs(i), self.derivatives):
+            if c != 0.0:
+                prev = prev + c * d
         prev = prev.to(sample.dtype)
         return {"prev_sample": prev} if return_dict else (prev,)

@@ -4,9 +4,10 @@ capture, get_token_maps (twice: colour masks, region masks), rich-text pass.
 
 Extra flags: --load_path (LOCAL diffusers-format directory; there is no hub access in this environment),
 --synthetic (random weights + random prompt embeddings, for smoke runs without checkpoints) and
---scheduler {default,ddim,dpmpp_2m,euler_a,unipc,heun} (default: PLMS for SD1.5, Euler for SDXL; DPM-Solver++(2M) is
-the usual choice at about 20 --sample_steps, UniPC the sampler built for 5-10; euler_a, Euler Ancestral, and heun,
-Heun's second-order method, which evaluates the UNet 2N - 1 times for N --sample_steps, are for SDXL / AnimeXL only).
+--scheduler {default,ddim,dpmpp_2m,euler_a,unipc,heun,lms} (default: PLMS for SD1.5, Euler for SDXL; DPM-Solver++(2M)
+is the usual choice at about 20 --sample_steps, UniPC the sampler built for 5-10; euler_a, Euler Ancestral, heun, Heun's
+second-order method, which evaluates the UNet 2N - 1 times for N --sample_steps, and lms, k-LMS, are for SDXL / AnimeXL
+only).
 """
 import argparse
 import json
@@ -23,7 +24,8 @@ from rtti_b200.attention_utils import get_token_maps  # noqa: E402
 from rtti_b200.region_diffusion import RegionDiffusion  # noqa: E402
 from rtti_b200.region_diffusion_sdxl import RegionDiffusionXL  # noqa: E402
 from rtti_b200.schedulers import (DDIMScheduler, DPMSolverMultistepScheduler,  # noqa: E402
-                                  EulerAncestralDiscreteScheduler, HeunDiscreteScheduler, UniPCMultistepScheduler)
+                                  EulerAncestralDiscreteScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler,
+                                  UniPCMultistepScheduler)
 from rtti_b200.richtext_utils import (get_attention_control_input, get_gradient_guidance_input,  # noqa: E402
                                       get_region_diffusion_input, parse_json, seed_everything)
 
@@ -40,7 +42,7 @@ def _save(img, path):
 def main(args, param):
     os.makedirs(args.run_dir, exist_ok=True)
     xl = args.model in ("SDXL", "AnimeXL")
-    if args.scheduler in ("euler_a", "heun") and not xl:
+    if args.scheduler in ("euler_a", "heun", "lms") and not xl:
         # the SD1.5 loop, like the reference's, never calls scale_model_input: the Euler family does not apply there
         raise SystemExit(f"--scheduler {args.scheduler} needs --model SDXL or AnimeXL: the SD1.5 sampler never scales the model "
                          "input, which the Euler schedulers require")
@@ -51,7 +53,7 @@ def main(args, param):
     if args.scheduler != "default":
         model.scheduler = {"ddim": DDIMScheduler, "dpmpp_2m": DPMSolverMultistepScheduler,
                            "euler_a": EulerAncestralDiscreteScheduler, "unipc": UniPCMultistepScheduler,
-                           "heun": HeunDiscreteScheduler}[args.scheduler]()
+                           "heun": HeunDiscreteScheduler, "lms": LMSDiscreteScheduler}[args.scheduler]()
 
     (base_prompt, style_prompts, footnote_prompts, footnote_targets, color_prompts, color_names, color_rgbs,
      sizes, use_grad_guidance) = parse_json(param["text_input"])
@@ -121,7 +123,7 @@ if __name__ == "__main__":
     p.add_argument("--inject_background", type=float, default=0.0)
     p.add_argument("--load_path", type=str, default=None)
     p.add_argument("--scheduler", type=str, default="default",
-                   choices=["default", "ddim", "dpmpp_2m", "euler_a", "unipc", "heun"])
+                   choices=["default", "ddim", "dpmpp_2m", "euler_a", "unipc", "heun", "lms"])
     a = p.parse_args()
     res = 512 if a.model == "SD" else 1024
     main(a, {"text_input": json.loads(a.rich_text_json), "height": a.height or res, "width": a.width or res,
