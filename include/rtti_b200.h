@@ -237,6 +237,28 @@ int rtti_region_blend_cfg_rescale_lms(const void* eps_uncond, const void* const*
                                       void* latents_out, float c0, float c1, float c2, float c3, const void* d1,
                                       const void* d2, const void* d3, float guidance_rescale, void* stream);
 
+/* Singlestep forms ("_ss") of the blend entry points, for DPM-Solver++(2S) (rich-text-to-image_b200/schedulers.py,
+ * DPMSolverSinglestepScheduler.singlestep_coeffs). They replace the scheduler step of
+ * models/region_diffusion_sdxl.py:837-846 and :908 with a DPMSolverSinglestepScheduler assigned to the reference's
+ * scheduler. The blend, CFG and rescale arithmetic is that of the Euler form; the update of the latents is, in fp32,
+ *   D  = hx * x + he * eps                              (written to d_out[n])
+ *   x' = cx * x + cd * D + cp * D_prev + cs * xs        (x' rounded to fp16)
+ * with x the fp16 latents, eps the fp16-rounded (rescaled) noise prediction written to eps_out, D_prev = d_prev[n]
+ * the D of the block's first step and xs[n] the fp16 latents that entered it. The multistep update is formed exactly as the
+ * "_ms" forms form it and cs * xs is added last; xs is read only when cs != 0, so with cs == 0 the result (latents_out,
+ * d_out and eps_out) equals the "_ms" form's bit for bit. latents, latents_out and d_out are required; d_prev may be
+ * null only when cp == 0 and may alias d_out; xs may be null only when cs == 0. d_prev / d_out / xs 16-byte aligned.
+ * The other checks are those of the Euler form; on any error nothing is launched. */
+int rtti_region_blend_cfg_ss(const void* eps_uncond, const void* const* eps_region, const float* masks, int n_regions,
+                             long long n, float guidance, void* eps_out, const void* latents, void* latents_out,
+                             float hx, float he, float cx, float cs, float cd, float cp, const float* d_prev,
+                             float* d_out, const void* xs, void* stream);
+int rtti_region_blend_cfg_rescale_ss(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                     int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                     void* latents_out, float hx, float he, float cx, float cs, float cd, float cp,
+                                     const float* d_prev, float* d_out, const void* xs, float guidance_rescale,
+                                     void* stream);
+
 /* Colour-guidance loss forward + analytic backward w.r.t. the VAE decoder output.
  * Replaces models/region_diffusion_sdxl.py:857-865 (clamp, masked mean RGB, MSE*100, autograd of those).
  *   decoded [3, hw] fp32 (VAE output before /2+0.5), masks [n_colors, hw] fp32 (channel 0 of
@@ -421,6 +443,27 @@ int rtti_gather_blend_step_rescale_lms(const void* const* peer_slots, void* cons
                                        float c1, float c2, float c3, const void* d1, const void* d2, const void* d3,
                                        const void* d1_ref, const void* d2_ref, const void* d3_ref, void* eps_ref_out,
                                        unsigned int step_id, float guidance_rescale, void* stream);
+
+/* Singlestep forms of rtti_gather_blend_step / rtti_gather_blend_step_rescale (the update of rtti_region_blend_cfg_ss;
+ * they replace models/region_diffusion_sdxl.py:837-846 with a DPMSolverSinglestepScheduler assigned to the reference's
+ * scheduler). The reference-latent trajectory, when latents_ref is given, is stepped with the same coefficients on its
+ * own state d_prev_ref -> d_out_ref and xs_ref (with the requirements of d_prev / d_out / xs). For the same noise
+ * predictions the outputs equal those of the single-GPU forms (the C/D pair: one region and a mask of ones) bit for
+ * bit, whatever the world size. Same protocol and slot layout as the Euler forms. */
+int rtti_gather_blend_step_ss(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                              const int* slot_owner, int n_slots, int n_regions, const float* masks, long long n,
+                              float guidance, void* eps_out, const void* latents, void* latents_out,
+                              const void* latents_ref, void* latents_ref_out, float hx, float he, float cx, float cs,
+                              float cd, float cp, const float* d_prev, float* d_out, const void* xs,
+                              const float* d_prev_ref, float* d_out_ref, const void* xs_ref, unsigned int step_id,
+                              void* stream);
+int rtti_gather_blend_step_rescale_ss(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                      const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                      long long n, float guidance, void* eps_out, const void* latents,
+                                      void* latents_out, const void* latents_ref, void* latents_ref_out, float hx,
+                                      float he, float cx, float cs, float cd, float cp, const float* d_prev,
+                                      float* d_out, const void* xs, const float* d_prev_ref, float* d_out_ref,
+                                      const void* xs_ref, unsigned int step_id, float guidance_rescale, void* stream);
 
 /* Stripe-parallel colour guidance (multi-GPU; new relative to the single-GPU reference, which back-propagates
  * through the batch-1 VAE decoder on one device: models/region_diffusion_sdxl.py:849-867). Every activation of

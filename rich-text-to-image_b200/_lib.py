@@ -111,6 +111,17 @@ SIGNATURES = {
     "rtti_gather_blend_step_rescale_lms": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int,
                                                    P_int, c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5
                                            + [c_float] * 4 + [c_void_p] * 7 + [ctypes.c_uint, c_float, c_void_p]),
+    "rtti_region_blend_cfg_ss": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
+                                         c_void_p, c_void_p] + [c_float] * 6 + [c_void_p] * 3 + [c_void_p]),
+    "rtti_region_blend_cfg_rescale_ss": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float,
+                                                 c_void_p, c_void_p, c_void_p] + [c_float] * 6 + [c_void_p] * 3
+                                         + [c_float, c_void_p]),
+    "rtti_gather_blend_step_ss": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int, c_int,
+                                          c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 6
+                                  + [c_void_p] * 6 + [ctypes.c_uint, c_void_p]),
+    "rtti_gather_blend_step_rescale_ss": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int,
+                                                  c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 6
+                                          + [c_void_p] * 6 + [ctypes.c_uint, c_float, c_void_p]),
     "rtti_gn32_silu_fwd_striped": (c_int, [c_void_p] * 7 + [c_int, c_ll, c_int, c_int, c_float, c_int,
                                            ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, ctypes.c_uint,
                                            c_void_p]),

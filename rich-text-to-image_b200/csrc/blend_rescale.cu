@@ -85,8 +85,13 @@ struct RescaleLmsParams : RescaleParams {
   __half* eps_ref_out;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun / LMS update of the main
-// (REF false) / reference (REF true) trajectory
+// the DPM-Solver++(2S) form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory
+struct RescaleSsParams : RescaleParams {
+  SsStep ss, ss_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun / LMS /
+// DPM-Solver++(2S) update of the main (REF false) / reference (REF true) trajectory
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleParams& p, long long, const float* e16, float* x) {
 #pragma unroll
@@ -111,6 +116,10 @@ __device__ __forceinline__ void rs_step(const RescaleHeunParams& p, long long v,
 template <bool REF>
 __device__ __forceinline__ void rs_step(const RescaleLmsParams& p, long long v, const float* e16, float* x) {
   lms_step8(REF ? p.ls_ref : p.ls, v, e16, x);
+}
+template <bool REF>
+__device__ __forceinline__ void rs_step(const RescaleSsParams& p, long long v, const float* e16, float* x) {
+  ss_step8(REF ? p.ss_ref : p.ss, v, e16, x);
 }
 
 // the output of the reference trajectory's prediction: only the Heun form (the ds of its first stage) and the LMS form
@@ -337,6 +346,14 @@ __global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
   blend_rescale_body<PEER>(p, cfg_s, sm);
 }
 
+template <bool PEER>
+__global__ void __cluster_dims__(RS_CL, 1, 1) __launch_bounds__(RS_THREADS, 1)
+    blend_rescale_ss_kernel(const __grid_constant__ RescaleSsParams p) {
+  extern __shared__ float4 cfg_s[];
+  __shared__ RescaleSmem sm;
+  blend_rescale_body<PEER>(p, cfg_s, sm);
+}
+
 // the kernel of each parameter type
 template <bool PEER>
 const void* rescale_kernel(const RescaleParams&) { return (const void*)blend_rescale_kernel<PEER>; }
@@ -350,6 +367,8 @@ template <bool PEER>
 const void* rescale_kernel(const RescaleHeunParams&) { return (const void*)blend_rescale_heun_kernel<PEER>; }
 template <bool PEER>
 const void* rescale_kernel(const RescaleLmsParams&) { return (const void*)blend_rescale_lms_kernel<PEER>; }
+template <bool PEER>
+const void* rescale_kernel(const RescaleSsParams&) { return (const void*)blend_rescale_ss_kernel<PEER>; }
 
 // threads per CTA and vectors per thread: a function of n only
 void rescale_plan(long long n, int& threads, int& vpt) {
@@ -379,6 +398,8 @@ int launch_rescale(P& p, void* stream) {
     blend_rescale_heun_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else if constexpr (std::is_same<P, RescaleLmsParams>::value)
     blend_rescale_lms_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
+  else if constexpr (std::is_same<P, RescaleSsParams>::value)
+    blend_rescale_ss_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   else
     blend_rescale_kernel<PEER><<<RS_CL, p.threads, (size_t)p.vpt * p.threads * 32, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
@@ -651,5 +672,41 @@ extern "C" int rtti_gather_blend_step_rescale_lms(const void* const* peer_slots,
   p.ls = LmsStep{c0, c1, c2, c3, (const __half*)d1, (const __half*)d2, (const __half*)d3};
   p.ls_ref = LmsStep{c0, c1, c2, c3, (const __half*)d1_ref, (const __half*)d2_ref, (const __half*)d3_ref};
   p.eps_ref_out = (__half*)eps_ref_out;
+  return launch_rescale<true>(p, stream);
+}
+
+extern "C" int rtti_region_blend_cfg_rescale_ss(const void* eps_uncond, const void* const* eps_region,
+                                                const float* masks, int n_regions, long long n, float guidance,
+                                                void* eps_out, const void* latents, void* latents_out, float hx,
+                                                float he, float cx, float cs, float cd, float cp, const float* d_prev,
+                                                float* d_out, const void* xs, float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleSsParams p{};
+  int rc = rescale_args(eps_uncond, eps_region, masks, n_regions, n, guidance, eps_out, latents, latents_out, p);
+  if (rc == RTTI_OK) rc = ss_step_args(cs, cp, xs, d_prev, d_out);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.ss = SsStep{MsStep{hx, he, cx, cd, cp, d_prev, d_out}, cs, (const __half*)xs};
+  return launch_rescale<false>(p, stream);
+}
+
+extern "C" int rtti_gather_blend_step_rescale_ss(const void* const* peer_slots, void* const* peer_flags, int world,
+                                                 int rank, const int* slot_owner, int n_slots, int n_regions,
+                                                 const float* masks, long long n, float guidance, void* eps_out,
+                                                 const void* latents, void* latents_out, const void* latents_ref,
+                                                 void* latents_ref_out, float hx, float he, float cx, float cs,
+                                                 float cd, float cp, const float* d_prev, float* d_out, const void* xs,
+                                                 const float* d_prev_ref, float* d_out_ref, const void* xs_ref,
+                                                 unsigned int step_id, float guidance_rescale, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  RescaleSsParams p{};
+  int rc = gather_rescale_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                               eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = ss_step_args(cs, cp, xs, d_prev, d_out);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = ss_step_args(cs, cp, xs_ref, d_prev_ref, d_out_ref);
+  if (rc != RTTI_OK) return rc;
+  p.phi = guidance_rescale;
+  p.ss = SsStep{MsStep{hx, he, cx, cd, cp, d_prev, d_out}, cs, (const __half*)xs};
+  p.ss_ref = SsStep{MsStep{hx, he, cx, cd, cp, d_prev_ref, d_out_ref}, cs, (const __half*)xs_ref};
   return launch_rescale<true>(p, stream);
 }

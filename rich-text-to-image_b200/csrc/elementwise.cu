@@ -344,7 +344,7 @@ __global__ void geglu_kernel(const __half* __restrict__ proj, __half* __restrict
 struct BlendPtrs { const __half* eps[16]; };
 
 // step policies (rtti_internal.h): Euler, the multistep update of MsStep, the ancestral update of AncStep, the UniPC
-// update of UniPCStep, the Heun update of HeunStep, or the LMS update of LmsStep
+// update of UniPCStep, the Heun update of HeunStep, the LMS update of LmsStep, or the DPM-Solver++(2S) update of SsStep
 struct EulerStep { float dt_sigma; };
 __device__ __forceinline__ void apply_step(const EulerStep& s, long long, const float* e16, float* x) {
 #pragma unroll
@@ -357,6 +357,7 @@ __device__ __forceinline__ void apply_step(const UniPCStep& s, long long v, cons
 }
 __device__ __forceinline__ void apply_step(const HeunStep& s, long long v, const float* e16, float* x) { heun_step8(s, v, e16, x); }
 __device__ __forceinline__ void apply_step(const LmsStep& s, long long v, const float* e16, float* x) { lms_step8(s, v, e16, x); }
+__device__ __forceinline__ void apply_step(const SsStep& s, long long v, const float* e16, float* x) { ss_step8(s, v, e16, x); }
 
 template <class Step>
 __device__ __forceinline__ void region_blend_body(const __half* __restrict__ eps_uncond, const BlendPtrs& ptrs,
@@ -435,6 +436,13 @@ __global__ void region_blend_lms_kernel(const __half* __restrict__ eps_uncond, B
                                         const float* __restrict__ masks, int n_regions, long long n, float guidance,
                                         __half* __restrict__ eps_out, const __half* __restrict__ latents,
                                         __half* __restrict__ latents_out, const LmsStep st) {
+  region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
+}
+
+__global__ void region_blend_ss_kernel(const __half* __restrict__ eps_uncond, BlendPtrs ptrs,
+                                       const float* __restrict__ masks, int n_regions, long long n, float guidance,
+                                       __half* __restrict__ eps_out, const __half* __restrict__ latents,
+                                       __half* __restrict__ latents_out, const SsStep st) {
   region_blend_body(eps_uncond, ptrs, masks, n_regions, n, guidance, eps_out, latents, latents_out, st);
 }
 
@@ -751,6 +759,22 @@ extern "C" int rtti_region_blend_cfg_lms(const void* eps_uncond, const void* con
   region_blend_lms_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
       (__half*)latents_out, LmsStep{c0, c1, c2, c3, (const __half*)d1, (const __half*)d2, (const __half*)d3});
+  return ok_or_cuda();
+}
+
+extern "C" int rtti_region_blend_cfg_ss(const void* eps_uncond, const void* const* eps_region, const float* masks,
+                                        int n_regions, long long n, float guidance, void* eps_out, const void* latents,
+                                        void* latents_out, float hx, float he, float cx, float cs, float cd, float cp,
+                                        const float* d_prev, float* d_out, const void* xs, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  BlendPtrs ptrs{};
+  int rc = region_blend_args(eps_uncond, eps_region, masks, n_regions, n, eps_out, latents, latents_out, ptrs);
+  if (rc == RTTI_OK) rc = ss_step_args(cs, cp, xs, d_prev, d_out);
+  if (rc != RTTI_OK) return rc;
+  const long long nv = n / 8;
+  region_blend_ss_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+      (const __half*)eps_uncond, ptrs, masks, n_regions, n, guidance, (__half*)eps_out, (const __half*)latents,
+      (__half*)latents_out, SsStep{MsStep{hx, he, cx, cd, cp, d_prev, d_out}, cs, (const __half*)xs});
   return ok_or_cuda();
 }
 

@@ -88,8 +88,13 @@ struct GatherBlendLmsParams : GatherBlendParams {
   __half* eps_ref_out;
 };
 
-// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun / LMS update of the
-// main / reference trajectory
+// the DPM-Solver++(2S) form: the parameters of the Euler form (dt_sigma unused) + the step of each trajectory
+struct GatherBlendSsParams : GatherBlendParams {
+  SsStep ss, ss_ref;
+};
+
+// step policies (rtti_internal.h): the Euler update, or the multistep / ancestral / UniPC / Heun / LMS /
+// DPM-Solver++(2S) update of the main / reference trajectory
 __device__ __forceinline__ void gb_step(const GatherBlendParams& p, bool, long long, const float* e16, float* x) {
 #pragma unroll
   for (int i = 0; i < 8; ++i) x[i] = fmaf(e16[i], p.dt_sigma, x[i]);
@@ -109,6 +114,9 @@ __device__ __forceinline__ void gb_step(const GatherBlendHeunParams& p, bool ref
 }
 __device__ __forceinline__ void gb_step(const GatherBlendLmsParams& p, bool ref, long long v, const float* e16, float* x) {
   lms_step8(ref ? p.ls_ref : p.ls, v, e16, x);
+}
+__device__ __forceinline__ void gb_step(const GatherBlendSsParams& p, bool ref, long long v, const float* e16, float* x) {
+  ss_step8(ref ? p.ss_ref : p.ss, v, e16, x);
 }
 
 // the reference trajectory's fp16 prediction: only the Heun form (the ds of its first stage) and the LMS form (the
@@ -212,6 +220,10 @@ __global__ void __launch_bounds__(128) gather_blend_heun_kernel(const GatherBlen
   gather_blend_body(p);
 }
 __global__ void __launch_bounds__(128) gather_blend_lms_kernel(const GatherBlendLmsParams p) {
+  GB_PUBLISH_AND_WAIT(p);
+  gather_blend_body(p);
+}
+__global__ void __launch_bounds__(128) gather_blend_ss_kernel(const GatherBlendSsParams p) {
   GB_PUBLISH_AND_WAIT(p);
   gather_blend_body(p);
 }
@@ -388,5 +400,29 @@ extern "C" int rtti_gather_blend_step_lms(const void* const* peer_slots, void* c
   p.eps_ref_out = (__half*)eps_ref_out;
   const long long nv = n / 8;
   gather_blend_lms_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
+  return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
+}
+
+extern "C" int rtti_gather_blend_step_ss(const void* const* peer_slots, void* const* peer_flags, int world, int rank,
+                                         const int* slot_owner, int n_slots, int n_regions, const float* masks,
+                                         long long n, float guidance, void* eps_out, const void* latents,
+                                         void* latents_out, const void* latents_ref, void* latents_ref_out, float hx,
+                                         float he, float cx, float cs, float cd, float cp, const float* d_prev,
+                                         float* d_out, const void* xs, const float* d_prev_ref, float* d_out_ref,
+                                         const void* xs_ref, unsigned int step_id, void* stream) {
+  if (!latents || !latents_out) return RTTI_ERR_ARG;
+  GatherBlendSsParams p{};
+  int rc = gather_blend_args(peer_slots, peer_flags, world, rank, slot_owner, n_slots, n_regions, masks, n, guidance,
+                             eps_out, latents, latents_out, latents_ref, latents_ref_out, step_id, p);
+  if (rc == RTTI_OK) rc = ss_step_args(cs, cp, xs, d_prev, d_out);
+  if (rc == RTTI_OK && latents_ref != nullptr) rc = ss_step_args(cs, cp, xs_ref, d_prev_ref, d_out_ref);
+  if (rc == RTTI_OK && (((uintptr_t)masks | (uintptr_t)eps_out | (uintptr_t)latents | (uintptr_t)latents_out |
+                         (uintptr_t)latents_ref | (uintptr_t)latents_ref_out) & 15))
+    rc = RTTI_ERR_ALIGN;
+  if (rc != RTTI_OK) return rc;
+  p.ss = SsStep{MsStep{hx, he, cx, cd, cp, d_prev, d_out}, cs, (const __half*)xs};
+  p.ss_ref = SsStep{MsStep{hx, he, cx, cd, cp, d_prev_ref, d_out_ref}, cs, (const __half*)xs_ref};
+  const long long nv = n / 8;
+  gather_blend_ss_kernel<<<(int)((nv + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
   return cudaGetLastError() == cudaSuccess ? RTTI_OK : RTTI_ERR_CUDA;
 }

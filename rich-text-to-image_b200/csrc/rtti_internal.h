@@ -57,6 +57,15 @@ inline int lms_step_args(float c1, float c2, float c3, const void* d1, const voi
   return (((uintptr_t)d1 | (uintptr_t)d2 | (uintptr_t)d3) & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
 }
 
+// the buffers of a singlestep (DPM-Solver++(2S)) blend step: those of the multistep step, and the block's starting
+// latents xs, required when cs != 0 and 16-byte aligned
+inline int ss_step_args(float cs, float cp, const void* xs, const float* d_prev, const float* d_out) {
+  const int rc = ms_step_args(cp, d_prev, d_out);
+  if (rc != RTTI_OK) return rc;
+  if (cs != 0.f && !xs) return RTTI_ERR_ARG;
+  return ((uintptr_t)xs & 15) ? RTTI_ERR_ALIGN : RTTI_OK;
+}
+
 #ifdef __CUDACC__
 // GroupNorm statistics of a set of values as (count n, mean, m2 = sum of squared deviations from the mean), merged with
 // the pairwise update of Chan, Golub & LeVeque. Unlike a one-pass E[x^2] - E[x]^2 in fp32, which loses about
@@ -267,6 +276,26 @@ __device__ __forceinline__ void lms_step8(const LmsStep& s, long long v, const f
   if (s.c1 != 0.f) lms_fma8(h1, s.c1, x);
   if (s.c2 != 0.f) lms_fma8(h2, s.c2, x);
   if (s.c3 != 0.f) lms_fma8(h3, s.c3, x);
+}
+
+// The DPM-Solver++(2S) update (schedulers.py, DPMSolverSinglestepScheduler.singlestep_coeffs), in fp32:
+//   D  = hx * x + he * eps                              written to d_out
+//   x' = cx * x + cd * D + cp * D_prev + cs * xs
+// with xs the fp16 [n] latents that entered the first step of the current two-step block: (hx, he, cx, cd, 0, 0) on a
+// first step, (hx, he, 0, cd, cp, cs) on the second. The multistep update is formed first, exactly as ms_step8 forms it
+// (d_prev may alias d_out), and cs * xs added last; xs is read (128-bit, issued before the multistep arithmetic) only
+// when cs != 0, so cs = 0 gives the multistep bits.
+struct SsStep {
+  MsStep ms;
+  float cs;
+  const __half* xs;
+};
+
+__device__ __forceinline__ void ss_step8(const SsStep& s, long long v, const float* e16, float* x) {
+  uint4 u;
+  if (s.cs != 0.f) u = *reinterpret_cast<const uint4*>(s.xs + v * 8);
+  ms_step8(s.ms, v, e16, x);
+  if (s.cs != 0.f) lms_fma8(u, s.cs, x);
 }
 
 // fixed-order tree over the 32 lanes of a warp; lane 0 ends with the statistics of every lane

@@ -400,6 +400,42 @@ class LMSStep:
         return a + ([_ptr(t) for t in self.d_ref] + [_ptr(self.eps_ref_out)] if ref else [])
 
 
+class SinglestepStep:
+    """The DPM-Solver++(2S) update of one blend call: `coeffs` (schedulers.SinglestepCoeffs: hx, he, cx, cs, cd, cp),
+    D = hx x + he eps, x' = cx x + cd D + cp D_prev + cs xs. d_prev / d_out: the fp32 [n] D buffers as in MultistepStep
+    (d_prev read when cp != 0, may be the same tensor as d_out); xs: the fp16 [n] latents that entered the block's first
+    step (read when cs != 0; may be None otherwise; only read, so no output may overlap it). d_prev_ref / d_out_ref /
+    xs_ref: the reference-latent trajectory's (gather_blend_step only)."""
+
+    def __init__(self, coeffs, d_prev, d_out, xs, d_prev_ref=None, d_out_ref=None, xs_ref=None):
+        self.coeffs = tuple(float(c) for c in coeffs)
+        if len(self.coeffs) != 6:
+            raise _lib.RttiError(f"singlestep blend: coeffs must be (hx, he, cx, cs, cd, cp), got {len(self.coeffs)} values")
+        self.main, self.ref = (d_prev, d_out, xs), (d_prev_ref, d_out_ref, xs_ref)
+
+    def _check(self, n, ref, outs=()):
+        """`outs`: the fp16 output tensors of the call, which must not overlap xs."""
+        _, _, _, cs, _, cp = self.coeffs
+        outs = [o for o in outs if o is not None]
+        for (d_prev, d_out, xs), sfx in [(self.main, "")] + ([(self.ref, "_ref")] if ref else []):
+            for t, need, dtype, name in ((d_prev, cp != 0.0, torch.float32, "d_prev"), (d_out, True, torch.float32, "d_out"),
+                                         (xs, cs != 0.0, _F16, "xs")):
+                if t is None:
+                    if need:
+                        raise _lib.RttiError(f"singlestep blend: {name}{sfx} is required")
+                    continue
+                _req(t, dtype, name + sfx)
+                if not t.is_contiguous() or t.numel() != n:
+                    raise _lib.RttiError(f"singlestep blend: {name}{sfx} must be a contiguous {dtype} tensor of {n} "
+                                         "elements")
+            if xs is not None and any(_overlap(xs, o) for o in outs):
+                raise _lib.RttiError(f"singlestep blend: xs{sfx} overlaps an output of the call")
+
+    def args(self, ref=False):
+        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(t) for t in self.main]
+        return a + ([_ptr(t) for t in self.ref] if ref else [])
+
+
 def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0,
                      step=None):
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
@@ -413,7 +449,8 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     used); a HeunStep — the Heun update (rtti_region_blend_cfg_heun / rtti_region_blend_cfg_rescale_heun; dt_sigma is
     not used, nor are xs_ref / ds_ref; eps_ref_out must be None); an LMSStep — the LMS update (rtti_region_blend_cfg_lms
     / rtti_region_blend_cfg_rescale_lms; dt_sigma is not used, nor are d1_ref / d2_ref / d3_ref; eps_ref_out must be
-    None)."""
+    None); a SinglestepStep — the DPM-Solver++(2S) update (rtti_region_blend_cfg_ss / rtti_region_blend_cfg_rescale_ss;
+    dt_sigma is not used, nor are the _ref buffers)."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -424,7 +461,20 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    if isinstance(step, LMSStep):
+    if isinstance(step, SinglestepStep):
+        if latents is None:
+            raise _lib.RttiError("region_blend_cfg: a singlestep step needs the latents")
+        step._check(n, False, (eps_out, lat_out))
+        if guidance_rescale == 0.0:
+            rc = lib.rtti_region_blend_cfg_ss(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                              _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_ss")
+        else:
+            rc = lib.rtti_region_blend_cfg_rescale_ss(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
+                                                      _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
+                                                      float(guidance_rescale), _stream())
+            _lib.check(rc, "rtti_region_blend_cfg_rescale_ss")
+    elif isinstance(step, LMSStep):
         if latents is None:
             raise _lib.RttiError("region_blend_cfg: an LMS step needs the latents")
         step._check(n, False, (eps_out, lat_out))
@@ -576,7 +626,9 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     (rtti_gather_blend_step_unipc / rtti_gather_blend_step_rescale_unipc); a HeunStep (with xs_ref / ds_ref, and
     optionally eps_ref_out, when latents_ref is given) — the Heun update (rtti_gather_blend_step_heun /
     rtti_gather_blend_step_rescale_heun); an LMSStep (with d1_ref / d2_ref / d3_ref, and optionally eps_ref_out, when
-    latents_ref is given) — the LMS update (rtti_gather_blend_step_lms / rtti_gather_blend_step_rescale_lms).
+    latents_ref is given) — the LMS update (rtti_gather_blend_step_lms / rtti_gather_blend_step_rescale_lms); a
+    SinglestepStep (with d_prev_ref / d_out_ref / xs_ref when latents_ref is given) — the DPM-Solver++(2S) update
+    (rtti_gather_blend_step_ss / rtti_gather_blend_step_rescale_ss).
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
@@ -587,7 +639,17 @@ def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_region
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    if isinstance(step, LMSStep):
+    if isinstance(step, SinglestepStep):
+        step._check(n, latents_ref is not None, (eps, lat_out, ref_out))
+        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
+                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
+        args += step.args(ref=True) + [int(step_id)]
+        if guidance_rescale == 0.0:
+            _lib.check(lib.rtti_gather_blend_step_ss(*args, _stream()), "rtti_gather_blend_step_ss")
+        else:
+            _lib.check(lib.rtti_gather_blend_step_rescale_ss(*args, float(guidance_rescale), _stream()),
+                       "rtti_gather_blend_step_rescale_ss")
+    elif isinstance(step, LMSStep):
         step._check(n, latents_ref is not None, (eps, lat_out, ref_out))
         args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
                 float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]

@@ -10,7 +10,9 @@ capture that overwrites instead of accumulating, :423), executed as one batched 
 `.scheduler` is PLMS (PNDMScheduler) by default and steps on the host; DDIMScheduler and DPMSolverMultistepScheduler
 (schedulers.py) step inside the fused blend kernels (rtti_region_blend_cfg_ms), with one fp32 history of the x0
 prediction per trajectory; UniPCMultistepScheduler steps inside rtti_region_blend_cfg_unipc, with three fp32 histories
-per trajectory (ops.UniPCHistory).
+per trajectory (ops.UniPCHistory); DPMSolverSinglestepScheduler (DPM-Solver++(2S)) steps inside
+rtti_region_blend_cfg_ss, with one fp32 history of the x0 prediction and the fp16 latents that entered the current
+two-step block per trajectory.
 """
 import math
 from typing import Optional
@@ -20,7 +22,7 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers, SelfAttentionLayers
-from .schedulers import MULTISTEP_SCHEDULERS, PNDMScheduler, UniPCMultistepScheduler
+from .schedulers import MULTISTEP_SCHEDULERS, DPMSolverSinglestepScheduler, PNDMScheduler, UniPCMultistepScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -111,7 +113,11 @@ class RegionDiffusion:
     @torch.no_grad()
     def produce_latents(self, text_embeddings, height=512, width=512, num_inference_steps=50, guidance_scale=7.5,
                         latents=None, use_guidance=False, text_format_dict={}, inject_selfattn=0, inject_background=0):
-        """:86-174. text_embeddings = [uncond, region_1..region_{N-1}, base]."""
+        """:86-174. text_embeddings = [uncond, region_1..region_{N-1}, base].
+        With DPMSolverSinglestepScheduler each trajectory keeps its x0 prediction and the latents that entered its
+        current two-step block; the second step of a block restarts from those latents, so colour guidance and
+        background injection applied after a first step reach the second step only through its prediction, as in the
+        reference with DPMSolverSinglestepScheduler assigned to its scheduler."""
         dev = self.device
         tfd = text_format_dict or {}
         if latents is None:
@@ -141,7 +147,9 @@ class RegionDiffusion:
         kv_caches = {}
         n_t = len(timesteps)
         multistep = isinstance(self.scheduler, MULTISTEP_SCHEDULERS)
-        if multistep:   # one x0-prediction history per trajectory (both are stepped on every step)
+        singlestep = isinstance(self.scheduler, DPMSolverSinglestepScheduler)
+        xs = xs_ref = None   # 2S: the latents that entered the current block's first step, per trajectory
+        if multistep or singlestep:   # one x0-prediction history per trajectory (both are stepped on every step)
             d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev)
             d_hist_ref = torch.empty_like(d_hist) if inject else None
         unipc = isinstance(self.scheduler, UniPCMultistepScheduler)
@@ -189,6 +197,19 @@ class RegionDiffusion:
                                                           latents=latents_ref.contiguous(),
                                                           step=ops.UniPCStep.of(c, up_hist_ref))
                     up_hist_ref.rotate()
+            elif singlestep:
+                c = self.scheduler.singlestep_coeffs(i)
+                lat, lat_ref = latents.contiguous(), (latents_ref.contiguous() if inject else None)
+                noise_pred, latents = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks,
+                                                           guidance_scale, latents=lat,
+                                                           step=ops.SinglestepStep(c, d_hist, d_hist, xs))
+                if inject:
+                    _, latents_ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
+                                                          [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale,
+                                                          latents=lat_ref,
+                                                          step=ops.SinglestepStep(c, d_hist_ref, d_hist_ref, xs_ref))
+                if self.scheduler.is_first_step(i):
+                    xs, xs_ref = lat, lat_ref
             else:
                 noise_pred = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks, guidance_scale)  # :119-132
                 if inject:                                                                                  # :134-143
@@ -221,7 +242,9 @@ class RegionDiffusion:
         kv = CrossKVCache()
         ones = torch.ones(1, latents[0].numel(), dtype=torch.float32, device=dev)
         multistep = isinstance(self.scheduler, MULTISTEP_SCHEDULERS)
-        d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev) if multistep else None
+        singlestep = isinstance(self.scheduler, DPMSolverSinglestepScheduler)
+        d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev) if multistep or singlestep else None
+        xs = None   # 2S: the latents that entered the current block's first step
         up_hist = ops.UniPCHistory(latents.numel(), dev) if isinstance(self.scheduler, UniPCMultistepScheduler) else None
         for i, t in enumerate(self.scheduler.timesteps):
             x = latents.expand(2, -1, -1, -1)
@@ -237,6 +260,14 @@ class RegionDiffusion:
                                                   latents=latents.contiguous(),
                                                   step=ops.UniPCStep.of(self.scheduler.unipc_coeffs(i), up_hist))
                 up_hist.rotate()
+                continue
+            if singlestep:
+                lat = latents.contiguous()
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=lat, step=ops.SinglestepStep(
+                                                      self.scheduler.singlestep_coeffs(i), d_hist, d_hist, xs))
+                if self.scheduler.is_first_step(i):
+                    xs = lat
                 continue
             noise_pred = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale)
             latents = self.scheduler.step(noise_pred, t, latents)["prev_sample"].to(torch.float16)

@@ -11,8 +11,9 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
     rtti_region_blend_cfg_rescale with guidance_rescale > 0; their "_ms" forms for DDIM / DPM-Solver++(2M), which
     keep one fp32 history of the x0 prediction per trajectory, "_anc" forms for Euler Ancestral, which add the
     noise drawn for the step, "_unipc" forms for UniPC, which keep three fp32 histories per trajectory, "_heun"
-    forms for Heun's method, which read the fp16 latents and prediction saved at the first stage, and "_lms" forms for
-    k-LMS, which read the fp16 predictions of the last three steps);
+    forms for Heun's method, which read the fp16 latents and prediction saved at the first stage, "_lms" forms for
+    k-LMS, which read the fp16 predictions of the last three steps, and "_ss" forms for DPM-Solver++(2S), which keep
+    one fp32 history of the x0 prediction per trajectory and read the fp16 latents that entered the two-step block);
     colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
@@ -26,8 +27,8 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
-from .schedulers import (MULTISTEP_SCHEDULERS, DDIMScheduler, EulerAncestralDiscreteScheduler, EulerDiscreteScheduler,
-                         HeunDiscreteScheduler, LMSDiscreteScheduler, UniPCMultistepScheduler)
+from .schedulers import (MULTISTEP_SCHEDULERS, DDIMScheduler, DPMSolverSinglestepScheduler, EulerAncestralDiscreteScheduler,
+                         EulerDiscreteScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler, UniPCMultistepScheduler)
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -41,8 +42,10 @@ def _step_kind(scheduler):
     """The fused update a scheduler runs as: "euler" (EulerDiscreteScheduler), "ancestral"
     (EulerAncestralDiscreteScheduler: the Euler update plus the noise term, ancestral_coeffs), "multistep"
     (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs), "unipc" (UniPCMultistepScheduler, unipc_coeffs),
-    "heun" (HeunDiscreteScheduler, heun_coeffs) or "lms" (LMSDiscreteScheduler, lms_coeffs). Any other scheduler has no
-    fused update here."""
+    "heun" (HeunDiscreteScheduler, heun_coeffs), "lms" (LMSDiscreteScheduler, lms_coeffs) or "singlestep"
+    (DPMSolverSinglestepScheduler, singlestep_coeffs). Any other scheduler has no fused update here."""
+    if isinstance(scheduler, DPMSolverSinglestepScheduler):
+        return "singlestep"
     if isinstance(scheduler, LMSDiscreteScheduler):
         return "lms"
     if isinstance(scheduler, HeunDiscreteScheduler):
@@ -57,7 +60,8 @@ def _step_kind(scheduler):
         return "multistep"
     raise TypeError(f"RegionDiffusionXL: unsupported scheduler {type(scheduler).__name__}; supported: "
                     "EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler, "
-                    "UniPCMultistepScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler (rtti_b200.schedulers)")
+                    "UniPCMultistepScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler, DPMSolverSinglestepScheduler "
+                    "(rtti_b200.schedulers)")
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -223,9 +227,9 @@ class RegionDiffusionXL:
         guidance_scale > 1) rescales the CFG prediction as diffusers' rescale_noise_cfg in both passes; the reference
         implements it for the plain pass only (:903-905) and raises NotImplementedError in the rich-text pass (:827-830).
         `self.scheduler` may be EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler,
-        DPMSolverMultistepScheduler, UniPCMultistepScheduler, HeunDiscreteScheduler or LMSDiscreteScheduler
-        (schedulers.py); `eta` > 0 (stochastic DDIM, which the reference's plain pass forwards to DDIM) is not
-        implemented.
+        DPMSolverMultistepScheduler, UniPCMultistepScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler or
+        DPMSolverSinglestepScheduler (schedulers.py); `eta` > 0 (stochastic DDIM, which the reference's plain pass
+        forwards to DDIM) is not implemented.
         With a multistep or UniPC scheduler the rich-text pass keeps one history per trajectory: where the reference
         steps the reference latents jointly with the main latents only on a prefix of the steps (inject_selfattn = 0,
         0 < inject_background < 1, :831-846) and then steps the main latents alone, the main latents keep their own
@@ -243,6 +247,13 @@ class RegionDiffusionXL:
         with the multistep schedulers, where the reference steps the reference latents jointly only on a prefix of the
         steps (inject_selfattn = 0, 0 < inject_background < 1), it would go on to add a batch-1 prediction to batch-2
         ones; here each trajectory keeps its own history.
+        With DPMSolverSinglestepScheduler (DPM-Solver++(2S)) the steps form blocks of two; each trajectory keeps one fp32
+        x0 prediction and the fp16 latents that entered its block's first step. The second step restarts from those
+        latents, so colour guidance and background injection applied after a first step reach the second step only
+        through its prediction, as in the reference with DPMSolverSinglestepScheduler assigned to its scheduler. Where
+        the reference steps the reference latents jointly only on a prefix of the steps (inject_selfattn = 0,
+        0 < inject_background < 1), here each trajectory keeps its own state; if the prefix ends after a first step, the
+        reference latents keep their first-step value, as with Heun and LMS.
         With EulerAncestralDiscreteScheduler the noise z of each step is drawn as diffusers' randn_tensor draws it, fp16,
         from `generator` when one is given (on its device: a CPU generator draws on the CPU), otherwise from the global
         RNG of the sampling device. The plain pass draws [1, ...] per step, as the reference does. The rich-text pass
@@ -310,7 +321,9 @@ class RegionDiffusionXL:
         i % callback_steps == 0 for the order-1 schedulers, only second stages and the last iteration for Heun.
         LMS: the UNet input is scaled as for Euler and the blend kernel takes the lms_coeffs(i) update on the fp16
         predictions of the last three steps (blend outputs, referenced while they are in the history; nothing writes
-        them in place)."""
+        them in place). DPM-Solver++(2S): the UNet sees the latents unscaled and the blend kernel takes the
+        singlestep_coeffs(i) update on one fp32 D buffer; a first step keeps the latents it stepped as the block's xs
+        (referenced until the second step reads them)."""
         phi = _rescale_phi(guidance_scale, guidance_rescale)
         ctx2 = torch.cat([ctx[:1], ctx[-1:]])
         pooled2 = torch.cat([pooled[:1], pooled[-1:]])
@@ -318,13 +331,15 @@ class RegionDiffusionXL:
         ones = None
         kind = _step_kind(self.scheduler)
         multistep = kind == "multistep"
-        d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=latents.device) if multistep else None
+        singlestep = kind == "singlestep"
+        d_hist = (torch.empty(latents.numel(), dtype=torch.float32, device=latents.device) if multistep or singlestep
+                  else None)
         up_hist = ops.UniPCHistory(latents.numel(), latents.device) if kind == "unipc" else None
         heun = kind == "heun"
-        xs = ds = None   # Heun: the latents and the prediction of the last first stage
+        xs = ds = None   # Heun: the latents and the prediction of the last first stage; 2S: xs, the block's latents
         lms_hist = (None, None, None)   # LMS: the predictions of the last three steps, newest first
         for i, t in enumerate(timesteps):
-            if multistep or up_hist is not None:
+            if multistep or singlestep or up_hist is not None:
                 x = latents.expand(2, -1, -1, -1)
             else:
                 sigma = self.scheduler.sigma_at(i) if heun else self.scheduler.sigma(t)
@@ -361,6 +376,14 @@ class RegionDiffusionXL:
                                                     latents=latents.contiguous(), guidance_rescale=phi,
                                                     step=ops.LMSStep(self.scheduler.lms_coeffs(i), *lms_hist))
                 lms_hist = (e16,) + lms_hist[:2]
+            elif singlestep:
+                lat = latents.contiguous()
+                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                  latents=lat, guidance_rescale=phi,
+                                                  step=ops.SinglestepStep(self.scheduler.singlestep_coeffs(i), d_hist,
+                                                                          d_hist, xs))
+                if self.scheduler.is_first_step(i):
+                    xs = lat
             else:
                 _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
                                                   latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
@@ -438,6 +461,13 @@ class RegionDiffusionXL:
         # LMS: the fp16 predictions of the last three steps per trajectory, newest first
         st.lms = kind == "lms"
         st.lms_main = st.lms_ref = (None, None, None)
+        # DPM-Solver++(2S): the D buffers of the multistep schedulers, and the fp16 latents that entered the current
+        # block's first step per trajectory (referenced until its second step)
+        st.singlestep = kind == "singlestep"
+        if st.singlestep:
+            st.d_hist = torch.empty(n, dtype=torch.float32, device=dev)
+            st.d_hist_ref = torch.empty(n, dtype=torch.float32, device=dev) if inject else None
+        st.ss_xs = st.ss_xs_ref = None
         return st
 
     def _unet_pass(self, st, x, t, local, feat_inject_step):
@@ -532,7 +562,7 @@ class RegionDiffusionXL:
         passes, kind, plan, N = st.passes, st.kind, st.plan, st.N
         feat_inject_step = bool(float(t) > (1 - st.inject_selfattn) * 1000)            # :782
         background_inject_step = i < st.inject_background * st.n_t                      # :783
-        if st.multistep or st.unipc:   # scale_model_input is the identity
+        if st.multistep or st.unipc or st.singlestep:   # scale_model_input is the identity
             scale = None
         else:
             sigma = self.scheduler.sigma_at(i) if st.heun else self.scheduler.sigma(t)
@@ -603,6 +633,18 @@ class RegionDiffusionXL:
             eps_ref = torch.empty_like(st.latents_ref) if step_ref and fused else None
             step = ops.LMSStep(c, *st.lms_main, *hist_ref, eps_ref)
             step_main, step_refl = ops.LMSStep(c, *st.lms_main), ops.LMSStep(c, *hist_ref)
+        elif st.singlestep:
+            # each trajectory steps on its own D buffer; a first step keeps the latents it steps as its block's xs
+            dt = 0.0
+            c = self.scheduler.singlestep_coeffs(i)
+            first = self.scheduler.is_first_step(i)
+            st.latents = lat_in = st.latents.contiguous()
+            if step_ref:
+                st.latents_ref = ref_in = st.latents_ref.contiguous()
+            xs_ref = st.ss_xs_ref if step_ref else None
+            step = ops.SinglestepStep(c, st.d_hist, st.d_hist, st.ss_xs, st.d_hist_ref, st.d_hist_ref, xs_ref)
+            step_main = ops.SinglestepStep(c, st.d_hist, st.d_hist, st.ss_xs)
+            step_refl = ops.SinglestepStep(c, st.d_hist_ref, st.d_hist_ref, xs_ref)
         else:
             dt = self.scheduler.dt(t)
             step = step_main = step_refl = None
@@ -650,6 +692,10 @@ class RegionDiffusionXL:
             st.heun_main = (lat_in, st.noise_pred)
             if step_ref:
                 st.heun_ref = (ref_in, eps_ref)
+        if st.singlestep and first:
+            st.ss_xs = lat_in
+            if step_ref:
+                st.ss_xs_ref = ref_in
         if st.lms:
             st.lms_main = (st.noise_pred,) + st.lms_main[:2]
             if step_ref:

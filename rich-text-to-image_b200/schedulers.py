@@ -14,7 +14,8 @@ UniPCMultistepScheduler (bh2, order 2, the few-step sampler) runs through the fu
 with `unipc_coeffs(i)`. HeunDiscreteScheduler (Heun's second-order method on Euler's sigma grid, two UNet evaluations
 per step) runs through the fused blend kernels of the SDXL sampler with `heun_coeffs(k)`. LMSDiscreteScheduler (k-LMS,
 the fourth-order linear multistep method on Euler's sigma grid) runs through the fused blend kernels of the SDXL sampler
-with `lms_coeffs(i)`.
+with `lms_coeffs(i)`. DPMSolverSinglestepScheduler (DPM-Solver++(2S), two-step blocks that restart from the latents
+that entered the block) runs through the fused blend kernels of both samplers with `singlestep_coeffs(i)`.
 """
 import math
 from typing import NamedTuple
@@ -296,6 +297,107 @@ class DPMSolverMultistepScheduler(_MultistepBase):
 
 
 MULTISTEP_SCHEDULERS = (DDIMScheduler, DPMSolverMultistepScheduler)
+
+
+# ---------------------------------------------------------------------------------------------------- singlestep
+class SinglestepCoeffs(NamedTuple):
+    """One step of DPM-Solver++(2S) in data-prediction form (float64, host):
+        D  = hx * x + he * eps                               (x0 prediction, as in StepCoeffs)
+        x' = cx * x + cd * D + cp * D_prev + cs * xs         (D_prev: the D of the block's first step; xs: the latents
+                                                              that entered it; cs = cp = 0 on a first step)
+    The blend kernels' singlestep entry points (rtti_*_ss) evaluate exactly this with eps = the fp16-rounded prediction."""
+    hx: float
+    he: float
+    cx: float
+    cs: float
+    cd: float
+    cp: float
+
+
+class DPMSolverSinglestepScheduler(_MultistepBase):
+    """DPM-Solver++(2S): algorithm_type="dpmsolver++", solver_order=2, solver_type="midpoint", lower_order_final=True,
+    no Karras sigmas, epsilon prediction, with the SD1.5 / SDXL betas — diffusers 0.18.2
+    (`schedulers/scheduling_dpmsolver_singlestep.py`), restated. PARITY UNPINNED: that source is not available here; the
+    conventions below are the definition.
+      timesteps: those of DPMSolverMultistepScheduler (linspace grid, duplicates removed); N = len(timesteps)
+      order list: [1, 2] * (N // 2), plus [1] when N is odd; step i goes from t_i = ts[i] to ts[i+1] (0 on the last
+      step). order = 1: one UNet evaluation per step, so a sampling loop's callback fires on every iteration.
+      D_i = (x_i - sigma_{t_i} eps_i) / alpha_{t_i}, with x_i the latents the UNet saw at step i
+      order 1 (the first step of a two-step block, s1 = t_i -> s0 = ts[i+1]): DPM-Solver-1,
+        x' = (sigma_s0 / sigma_s1) x_i - alpha_s0 expm1(-h) D_i;  the block keeps xs = x_i and D_i
+      order 2 (the second step, s0 = t_i, from s1 = ts[i-1] to t = ts[i+1]): h = lambda_t - lambda_s1,
+        r0 = (lambda_s0 - lambda_s1) / h,
+        x' = (sigma_t / sigma_s1) xs - alpha_t expm1(-h) D_{i-1} - alpha_t expm1(-h) (D_i - D_{i-1}) / (2 r0)
+    The second step restarts from xs, the latents that entered the block: the current latents x_i reach it only through
+    eps_i (in D_i). Whatever a sampling loop does to the latents after a first step (colour guidance, background
+    injection) therefore acts on the second step's update through the prediction alone, as in diffusers. The samplers run
+    it through the fused blend kernels with the coefficients of `singlestep_coeffs(i)`, one fp32 D buffer and the fp16
+    xs per trajectory (ops.SinglestepStep); `step` is the stateful torch form in diffusers' calling convention. Not a
+    subclass of DPMSolverMultistepScheduler: the samplers dispatch on the class, and this update is not 2M's."""
+    _defaults = dict(num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012, beta_schedule="scaled_linear",
+                     trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                     dynamic_thresholding_ratio=0.995, sample_max_value=1.0, algorithm_type="dpmsolver++",
+                     solver_type="midpoint", lower_order_final=True, use_karras_sigmas=False,
+                     lambda_min_clipped=-float("inf"), variance_type=None)
+    _unsupported = dict(trained_betas=None, solver_order=2, prediction_type="epsilon", thresholding=False,
+                        algorithm_type="dpmsolver++", solver_type="midpoint", lower_order_final=True,
+                        use_karras_sigmas=False, lambda_min_clipped=-float("inf"), variance_type=None)
+
+    def __init__(self, **kw):
+        if kw.get("solver_type") in ("bh1", "bh2", "logrho"):
+            kw["solver_type"] = "midpoint"   # as diffusers does, so that from_config(UniPCMultistepScheduler) works
+        super().__init__(**kw)
+        self.order_list = []
+        self._xs = None
+
+    @staticmethod
+    def get_order_list(n):
+        """The order of each of n steps: [1, 2] * (n // 2), plus [1] when n is odd."""
+        return [1, 2] * (n // 2) + [1] * (n % 2)
+
+    def set_timesteps(self, num_inference_steps, device=None):
+        DPMSolverMultistepScheduler.set_timesteps(self, num_inference_steps, device)
+        self.order_list = self.get_order_list(len(self.timesteps_host))
+        self._xs = None
+
+    def is_first_step(self, i):
+        """Whether step i is first order: it starts a two-step block (or is the odd last step), so its input latents
+        become the xs of the block."""
+        return self.order_list[i] == 1
+
+    def singlestep_coeffs(self, i):
+        ts, n = self.timesteps_host, len(self.timesteps_host)
+        t_i = int(ts[i])
+        s = 0 if i == n - 1 else int(ts[i + 1])
+        hx, he, cx, cd, _ = self._first_order(t_i, s)
+        if self.order_list[i] == 1:
+            return SinglestepCoeffs(hx, he, cx, 0.0, cd, 0.0)
+        s1 = int(ts[i - 1])
+        lam = self._lambda
+        h = float(lam[s] - lam[s1])
+        r0 = float(lam[t_i] - lam[s1]) / h
+        a_t, em = float(self._alpha[s]), math.expm1(-h)
+        cs = float(self._sigma[s] / self._sigma[s1])
+        return SinglestepCoeffs(hx, he, 0.0, cs, -0.5 * a_t * em / r0, -a_t * em * (1.0 - 0.5 / r0))
+
+    def step(self, model_output, timestep, sample, return_dict=True, **kw):
+        """Stateful torch form of singlestep_coeffs in diffusers' calling convention (the samplers use the fused kernels
+        instead), in the precision of `sample` and at least fp32: a first step keeps `sample` as xs and its D."""
+        i = self.index_of(timestep)
+        c = self.singlestep_coeffs(i)
+        dt = torch.promote_types(sample.dtype, torch.float32)
+        x, e = sample.to(dt), model_output.to(dt)
+        d = c.hx * x + c.he * e
+        prev = c.cx * x + c.cd * d
+        if c.cp != 0.0:
+            prev = prev + c.cp * self._d_prev
+        if c.cs != 0.0:
+            prev = prev + c.cs * self._xs.to(dt)
+        if self.is_first_step(i):
+            self._xs = sample
+        self._d_prev = d
+        prev = prev.to(sample.dtype)
+        return {"prev_sample": prev} if return_dict else (prev,)
 
 
 # ---------------------------------------------------------------------------------------------------- UniPC

@@ -4,8 +4,9 @@ capture, get_token_maps (twice: colour masks, region masks), rich-text pass.
 
 Extra flags: --load_path (LOCAL diffusers-format directory; there is no hub access in this environment),
 --synthetic (random weights + random prompt embeddings, for smoke runs without checkpoints) and
---scheduler {default,ddim,dpmpp_2m,euler_a,unipc,heun,lms} (default: PLMS for SD1.5, Euler for SDXL; DPM-Solver++(2M)
-is the usual choice at about 20 --sample_steps, UniPC the sampler built for 5-10; euler_a, Euler Ancestral, heun, Heun's
+--scheduler {default,ddim,dpmpp_2m,dpmpp_2s,euler_a,unipc,heun,lms} (default: PLMS for SD1.5, Euler for SDXL;
+DPM-Solver++(2M) is the usual choice at about 20 --sample_steps, UniPC the sampler built for 5-10, dpmpp_2s
+DPM-Solver++(2S), the singlestep variant; euler_a, Euler Ancestral, heun, Heun's
 second-order method, which evaluates the UNet 2N - 1 times for N --sample_steps, and lms, k-LMS, are for SDXL / AnimeXL
 only).
 """
@@ -23,7 +24,7 @@ sys.path.insert(0, ROOT)
 from rtti_b200.attention_utils import get_token_maps  # noqa: E402
 from rtti_b200.region_diffusion import RegionDiffusion  # noqa: E402
 from rtti_b200.region_diffusion_sdxl import RegionDiffusionXL  # noqa: E402
-from rtti_b200.schedulers import (DDIMScheduler, DPMSolverMultistepScheduler,  # noqa: E402
+from rtti_b200.schedulers import (DDIMScheduler, DPMSolverMultistepScheduler, DPMSolverSinglestepScheduler,  # noqa: E402
                                   EulerAncestralDiscreteScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler,
                                   UniPCMultistepScheduler)
 from rtti_b200.richtext_utils import (get_attention_control_input, get_gradient_guidance_input,  # noqa: E402
@@ -52,6 +53,7 @@ def main(args, param):
     model = RegionDiffusionXL(load_path=args.load_path) if xl else RegionDiffusion("cuda", load_path=args.load_path)
     if args.scheduler != "default":
         model.scheduler = {"ddim": DDIMScheduler, "dpmpp_2m": DPMSolverMultistepScheduler,
+                           "dpmpp_2s": DPMSolverSinglestepScheduler,
                            "euler_a": EulerAncestralDiscreteScheduler, "unipc": UniPCMultistepScheduler,
                            "heun": HeunDiscreteScheduler, "lms": LMSDiscreteScheduler}[args.scheduler]()
 
@@ -123,7 +125,7 @@ if __name__ == "__main__":
     p.add_argument("--inject_background", type=float, default=0.0)
     p.add_argument("--load_path", type=str, default=None)
     p.add_argument("--scheduler", type=str, default="default",
-                   choices=["default", "ddim", "dpmpp_2m", "euler_a", "unipc", "heun", "lms"])
+                   choices=["default", "ddim", "dpmpp_2m", "dpmpp_2s", "euler_a", "unipc", "heun", "lms"])
     a = p.parse_args()
     res = 512 if a.model == "SD" else 1024
     main(a, {"text_input": json.loads(a.rich_text_json), "height": a.height or res, "width": a.width or res,
