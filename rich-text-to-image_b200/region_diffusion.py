@@ -22,12 +22,13 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers, SelfAttentionLayers
+from .lora import LoraLoaderMixin
 from .schedulers import MULTISTEP_SCHEDULERS, DPMSolverSinglestepScheduler, PNDMScheduler, UniPCMultistepScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
 
-class RegionDiffusion:
+class RegionDiffusion(LoraLoaderMixin):
     def __init__(self, device="cuda", unet=None, vae=None, text_encoder=None, load_path="runwayml/stable-diffusion-v1-5"):
         self.device = torch.device(device)
         torch.backends.cudnn.benchmark = True   # static shapes: let cuDNN pick its fastest conv algorithm once
@@ -55,6 +56,9 @@ class RegionDiffusion:
         unet.finalize(device).init_synthetic(seed)
         vae = AutoencoderKLDecoder(vae_cfg or VAEConfig.sd15()).init_synthetic(seed + 1).finalize(device) if with_vae else None
         return cls(device=device, unet=unet, vae=vae)
+
+    def _lora_components(self):
+        return self.unet, (() if self.text_encoder is None else (self.text_encoder.text_encoder,))
 
     # ------------------------------------------------------------------ capture API (:397-450)
     def register_tokenmap_hooks(self):

@@ -27,6 +27,7 @@ import torch
 
 from . import ops, region_parallel, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
+from .lora import LoraLoaderMixin
 from .schedulers import (MULTISTEP_SCHEDULERS, DDIMScheduler, DPMSolverSinglestepScheduler, EulerAncestralDiscreteScheduler,
                          EulerDiscreteScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler, UniPCMultistepScheduler)
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
@@ -70,7 +71,7 @@ class StableDiffusionXLPipelineOutput(dict):
         self.images = images
 
 
-class RegionDiffusionXL:
+class RegionDiffusionXL(LoraLoaderMixin):
     def __init__(self, load_path: str = "stabilityai/stable-diffusion-xl-base-1.0", device: str = "cuda",
                  force_zeros_for_empty_prompt: bool = True, unet=None, vae=None, scheduler=None,
                  text_encoders=None):
@@ -139,6 +140,10 @@ class RegionDiffusionXL:
         self.selfattn_maps = None
         self.crossattn_maps = None
         self.n_maps = None
+
+    def _lora_components(self):
+        te = self.text_encoders
+        return self.unet, (() if te is None else (te.text_encoder, te.text_encoder_2))
 
     # ------------------------------------------------------------------ helpers
     def encode_prompt(self, prompt, negative_prompt):
@@ -262,7 +267,12 @@ class RegionDiffusionXL:
         which passes no generator to the rich-text pass's step, that pass also draws from `generator`: a seeded run is
         reproducible from start to end. With generator=None both passes draw exactly what the reference draws. On more
         than one GPU every rank must add the same noise: sample() compares a digest of the noise source's state over
-        the ranks once and raises on every rank if they disagree."""
+        the ranks once and raises on every rank if they disagree.
+        `cross_attention_kwargs={"scale": s}` with a LoRA loaded (load_lora_weights) re-merges it at scale s before the
+        prompt is encoded, so the UNet and both text encoders use s. Unlike diffusers, where a call without the keyword
+        runs at scale 1.0, the scale stays in effect for later calls. With no LoRA loaded the argument is ignored."""
+        if cross_attention_kwargs and "scale" in cross_attention_kwargs and self._lora is not None:
+            self.set_lora_scale(cross_attention_kwargs["scale"])
         kind = _step_kind(self.scheduler)
         multistep = kind == "multistep"
         if multistep and eta > 0 and not run_rich_text and isinstance(self.scheduler, DDIMScheduler):

@@ -8,7 +8,8 @@ Extra flags: --load_path (LOCAL diffusers-format directory; there is no hub acce
 DPM-Solver++(2M) is the usual choice at about 20 --sample_steps, UniPC the sampler built for 5-10, dpmpp_2s
 DPM-Solver++(2S), the singlestep variant; euler_a, Euler Ancestral, heun, Heun's
 second-order method, which evaluates the UNet 2N - 1 times for N --sample_steps, and lms, k-LMS, are for SDXL / AnimeXL
-only).
+only), --lora_path (a LOCAL LoRA .safetensors file, kohya or diffusers format, merged into the UNet and text-encoder
+weights) with --lora_scale (default 1.0).
 """
 import argparse
 import json
@@ -56,6 +57,8 @@ def main(args, param):
                            "dpmpp_2s": DPMSolverSinglestepScheduler,
                            "euler_a": EulerAncestralDiscreteScheduler, "unipc": UniPCMultistepScheduler,
                            "heun": HeunDiscreteScheduler, "lms": LMSDiscreteScheduler}[args.scheduler]()
+    if args.lora_path is not None:
+        model.load_lora_weights(args.lora_path, scale=args.lora_scale)
 
     (base_prompt, style_prompts, footnote_prompts, footnote_targets, color_prompts, color_names, color_rgbs,
      sizes, use_grad_guidance) = parse_json(param["text_input"])
@@ -126,6 +129,8 @@ if __name__ == "__main__":
     p.add_argument("--load_path", type=str, default=None)
     p.add_argument("--scheduler", type=str, default="default",
                    choices=["default", "ddim", "dpmpp_2m", "dpmpp_2s", "euler_a", "unipc", "heun", "lms"])
+    p.add_argument("--lora_path", type=str, default=None)
+    p.add_argument("--lora_scale", type=float, default=1.0)
     a = p.parse_args()
     res = 512 if a.model == "SD" else 1024
     main(a, {"text_input": json.loads(a.rich_text_json), "height": a.height or res, "width": a.width or res,
