@@ -35,8 +35,6 @@ SIGNATURES = {
     "rtti_add_bias_layernorm_fwd": (c_int, [c_void_p] * 7 + [c_int, c_int, c_float, c_void_p]),
     "rtti_ff_geglu_fwd": (c_int, [c_void_p] * 4 + [c_ll, c_int, c_int, c_void_p]),
     "rtti_geglu_fwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
-    "rtti_region_blend_cfg": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                      c_void_p, c_void_p, c_float, c_void_p]),
     "rtti_color_loss_workspace_elems": (c_ll, [c_int, c_ll]),
     "rtti_color_loss_fwd_bwd": (c_int, [c_void_p] * 3 + [c_int, c_ll] + [c_void_p] * 4),
     "rtti_latent_guidance_update": (c_int, [c_void_p] * 3 + [c_float, c_void_p, c_ll, c_void_p]),
@@ -48,80 +46,6 @@ SIGNATURES = {
     "rtti_add_bias_f32": (c_int, [c_void_p] * 4 + [c_ll, c_int, c_void_p]),
     "rtti_upsample_phase_interleave": (c_int, [c_void_p] * 3 + [c_int] * 4 + [c_void_p]),
     "rtti_upsample_phase_scatter": (c_int, [c_void_p] * 2 + [c_int] * 4 + [c_void_p]),
-    "rtti_gather_blend_step": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int, c_int, c_int,
-                                       c_void_p, c_ll, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_float,
-                                       ctypes.c_uint, c_void_p]),
-    "rtti_region_blend_cfg_rescale": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                              c_void_p, c_void_p, c_float, c_float, c_void_p]),
-    "rtti_gather_blend_step_rescale": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int, c_int,
-                                               c_int, c_void_p, c_ll, c_float, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                               c_float, ctypes.c_uint, c_float, c_void_p]),
-    "rtti_region_blend_cfg_ms": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                         c_void_p, c_void_p] + [c_float] * 5 + [c_void_p, c_void_p, c_void_p]),
-    "rtti_region_blend_cfg_rescale_ms": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float,
-                                                 c_void_p, c_void_p, c_void_p] + [c_float] * 5
-                                         + [c_void_p, c_void_p, c_float, c_void_p]),
-    "rtti_gather_blend_step_ms": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int, c_int,
-                                          c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 5
-                                  + [c_void_p] * 4 + [ctypes.c_uint, c_void_p]),
-    "rtti_gather_blend_step_rescale_ms": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int,
-                                                  c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 5
-                                          + [c_void_p] * 4 + [ctypes.c_uint, c_float, c_void_p]),
-    "rtti_region_blend_cfg_anc": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                          c_void_p, c_void_p, c_float, c_float, c_void_p, c_void_p]),
-    "rtti_region_blend_cfg_rescale_anc": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float,
-                                                  c_void_p, c_void_p, c_void_p, c_float, c_float, c_void_p, c_float,
-                                                  c_void_p]),
-    "rtti_gather_blend_step_anc": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int, c_int,
-                                           c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float, c_float]
-                                   + [c_void_p] * 2 + [ctypes.c_uint, c_void_p]),
-    "rtti_gather_blend_step_rescale_anc": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int,
-                                                   c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5
-                                           + [c_float, c_float] + [c_void_p] * 2 + [ctypes.c_uint, c_float, c_void_p]),
-    "rtti_region_blend_cfg_unipc": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                            c_void_p, c_void_p] + [c_float] * 10 + [c_void_p] * 5 + [c_void_p]),
-    "rtti_region_blend_cfg_rescale_unipc": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float,
-                                                    c_void_p, c_void_p, c_void_p] + [c_float] * 10 + [c_void_p] * 5
-                                            + [c_float, c_void_p]),
-    "rtti_gather_blend_step_unipc": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int,
-                                             c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 10
-                                     + [c_void_p] * 10 + [ctypes.c_uint, c_void_p]),
-    "rtti_gather_blend_step_rescale_unipc": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int,
-                                                     P_int, c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5
-                                             + [c_float] * 10 + [c_void_p] * 10 + [ctypes.c_uint, c_float, c_void_p]),
-    "rtti_region_blend_cfg_heun": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                           c_void_p, c_void_p] + [c_float] * 4 + [c_void_p] * 2 + [c_void_p]),
-    "rtti_region_blend_cfg_rescale_heun": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float,
-                                                   c_void_p, c_void_p, c_void_p] + [c_float] * 4 + [c_void_p] * 2
-                                           + [c_float, c_void_p]),
-    "rtti_gather_blend_step_heun": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int,
-                                            c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 4
-                                    + [c_void_p] * 5 + [ctypes.c_uint, c_void_p]),
-    "rtti_gather_blend_step_rescale_heun": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int,
-                                                    P_int, c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5
-                                            + [c_float] * 4 + [c_void_p] * 5 + [ctypes.c_uint, c_float, c_void_p]),
-    "rtti_region_blend_cfg_lms": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                          c_void_p, c_void_p] + [c_float] * 4 + [c_void_p] * 3 + [c_void_p]),
-    "rtti_region_blend_cfg_rescale_lms": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float,
-                                                  c_void_p, c_void_p, c_void_p] + [c_float] * 4 + [c_void_p] * 3
-                                          + [c_float, c_void_p]),
-    "rtti_gather_blend_step_lms": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int,
-                                           c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 4
-                                   + [c_void_p] * 7 + [ctypes.c_uint, c_void_p]),
-    "rtti_gather_blend_step_rescale_lms": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int,
-                                                   P_int, c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5
-                                           + [c_float] * 4 + [c_void_p] * 7 + [ctypes.c_uint, c_float, c_void_p]),
-    "rtti_region_blend_cfg_ss": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float, c_void_p,
-                                         c_void_p, c_void_p] + [c_float] * 6 + [c_void_p] * 3 + [c_void_p]),
-    "rtti_region_blend_cfg_rescale_ss": (c_int, [c_void_p, ctypes.POINTER(c_void_p), c_void_p, c_int, c_ll, c_float,
-                                                 c_void_p, c_void_p, c_void_p] + [c_float] * 6 + [c_void_p] * 3
-                                         + [c_float, c_void_p]),
-    "rtti_gather_blend_step_ss": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int, c_int,
-                                          c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 6
-                                  + [c_void_p] * 6 + [ctypes.c_uint, c_void_p]),
-    "rtti_gather_blend_step_rescale_ss": (c_int, [ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, P_int,
-                                                  c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5 + [c_float] * 6
-                                          + [c_void_p] * 6 + [ctypes.c_uint, c_float, c_void_p]),
     "rtti_gn32_silu_fwd_striped": (c_int, [c_void_p] * 7 + [c_int, c_ll, c_int, c_int, c_float, c_int,
                                            ctypes.POINTER(c_void_p), ctypes.POINTER(c_void_p), c_int, c_int, ctypes.c_uint,
                                            c_void_p]),
@@ -136,6 +60,23 @@ SIGNATURES = {
     "rtti_kmeans_fit": (c_int, [c_void_p, c_void_p] + [c_int] * 4 + [ctypes.c_double] + [c_void_p] * 5),
     "rtti_kmeans_supported": (c_int, [c_int, c_int]),
 }
+
+# The region-blend entry points: one form per fused scheduler update, as (suffix, float count, pointer count of the
+# main trajectory, pointer count of the reference trajectory). The update's floats and pointers follow the base
+# arguments; gather_blend_step also takes the reference trajectory's pointers and the step id. Each form comes with
+# and without the CFG rescale, whose φ is the last argument before the stream.
+BLEND_FORMS = (("", 1, 0, 0), ("_ms", 5, 2, 2), ("_anc", 2, 1, 1), ("_unipc", 10, 5, 5), ("_heun", 4, 2, 3),
+               ("_lms", 4, 3, 4), ("_ss", 6, 3, 3))
+_P_void = ctypes.POINTER(c_void_p)
+_BLEND_BASE = [c_void_p, _P_void, c_void_p, c_int, c_ll, c_float, c_void_p, c_void_p, c_void_p]
+_GATHER_BASE = [_P_void, _P_void, c_int, c_int, P_int, c_int, c_int, c_void_p, c_ll, c_float] + [c_void_p] * 5
+for _sfx, _nf, _np, _nr in BLEND_FORMS:
+    for _rescale in ("", "_rescale"):
+        _phi = [c_float] if _rescale else []
+        SIGNATURES[f"rtti_region_blend_cfg{_rescale}{_sfx}"] = (
+            c_int, _BLEND_BASE + [c_float] * _nf + [c_void_p] * _np + _phi + [c_void_p])
+        SIGNATURES[f"rtti_gather_blend_step{_rescale}{_sfx}"] = (
+            c_int, _GATHER_BASE + [c_float] * _nf + [c_void_p] * (_np + _nr) + [ctypes.c_uint] + _phi + [c_void_p])
 
 _lib = None
 

@@ -220,55 +220,104 @@ def geglu(proj, out=None):
     return out
 
 
-class MultistepStep:
+_DTYPE_NAME = {torch.float32: "fp32", _F16: "fp16"}
+
+
+def _overlap(a, b):
+    """Whether the storage spans of two tensors intersect."""
+    a0, b0 = a.data_ptr(), b.data_ptr()
+    return a0 < b0 + b.numel() * b.element_size() and b0 < a0 + a.numel() * a.element_size()
+
+
+class _Step:
+    """The fused scheduler update of one blend call: its floats `coeffs`, the [n] buffers of the main trajectory and
+    those of the reference-latent trajectory (gather_blend_step only), in the order the entry points take them. `form`
+    is the suffix of the entry points that run the update (_lib.BLEND_FORMS)."""
+    form = ""
+    what = ""               # the update's name in error messages
+    coeff_names = None      # when given, the number of coeffs is checked
+    names = dtypes = ()     # per buffer of one trajectory
+    read_only = ()          # buffers the update only reads: no output of the call may overlap them
+    has_eps_ref_out = False
+
+    def __init__(self, coeffs, main=(), ref=None, eps_ref_out=None):
+        self.coeffs = tuple(float(c) for c in coeffs)
+        if self.coeff_names and len(self.coeffs) != len(self.coeff_names):
+            raise _lib.RttiError(f"{self.what} blend: coeffs must be ({', '.join(self.coeff_names)}), got "
+                                 f"{len(self.coeffs)} values")
+        self.main = tuple(main)
+        self.ref = tuple(ref) if ref is not None else (None,) * len(self.main)
+        self.eps_ref_out = eps_ref_out
+
+    def _needed(self):
+        """Per buffer of one trajectory: whether this step reads or writes it (it may be None otherwise)."""
+        return ()
+
+    def _check(self, n, ref, outs=()):
+        """Refuse a missing or malformed buffer. `outs`: the output tensors of the call."""
+        if self.eps_ref_out is not None and not ref:
+            raise _lib.RttiError(f"{self.what} blend: eps_ref_out needs the reference latents")
+        need = self._needed()
+        items = list(zip(self.main, need, self.dtypes, self.names))
+        if ref:
+            items += [(t, nd, dt, name + "_ref") for t, nd, dt, name in zip(self.ref, need, self.dtypes, self.names)]
+            if self.has_eps_ref_out:
+                items.append((self.eps_ref_out, False, _F16, "eps_ref_out"))
+                outs = (*outs, self.eps_ref_out)
+        outs = [o for o in outs if o is not None]
+        for t, nd, dtype, name in items:
+            if t is None:
+                if nd:
+                    raise _lib.RttiError(f"{self.what} blend: {name} is required")
+                continue
+            _req(t, dtype, name)
+            if not t.is_contiguous() or t.numel() != n:
+                raise _lib.RttiError(f"{self.what} blend: {name} must be a contiguous {_DTYPE_NAME[dtype]} tensor of "
+                                     f"{n} elements")
+            if name.removesuffix("_ref") in self.read_only and any(_overlap(t, o) for o in outs):
+                raise _lib.RttiError(f"{self.what} blend: {name} overlaps an output of the call")
+
+    def args(self, ref=False):
+        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(t) for t in self.main]
+        if ref:
+            a += [_ptr(t) for t in self.ref] + ([_ptr(self.eps_ref_out)] if self.has_eps_ref_out else [])
+        return a
+
+
+class EulerStep(_Step):
+    """The Euler update of one blend call: x' = x + dt eps, with dt = sigma_next - sigma (EulerDiscreteScheduler.dt);
+    both trajectories take the same dt."""
+    what = "Euler"
+
+    def __init__(self, dt):
+        super().__init__((dt,))
+
+
+class MultistepStep(_Step):
     """The multistep (DDIM / DPM-Solver++) update of one blend call: `coeffs` (schedulers.StepCoeffs: hx, he, cx, cd, cp)
     and the fp32 histories of D = hx x + he eps, [n] each: d_prev (read when cp != 0; may be the same tensor as d_out)
     and d_out (written). d_prev_ref / d_out_ref: the reference-latent trajectory's (gather_blend_step only)."""
+    form, what, names, dtypes = "_ms", "multistep", ("d_prev", "d_out"), (torch.float32,) * 2
 
     def __init__(self, coeffs, d_prev, d_out, d_prev_ref=None, d_out_ref=None):
-        self.coeffs = tuple(float(c) for c in coeffs)
-        self.d_prev, self.d_out, self.d_prev_ref, self.d_out_ref = d_prev, d_out, d_prev_ref, d_out_ref
+        super().__init__(coeffs, (d_prev, d_out), (d_prev_ref, d_out_ref))
 
-    def _check(self, n, ref):
-        pairs = [(self.d_prev, self.d_out)] + ([(self.d_prev_ref, self.d_out_ref)] if ref else [])
-        for prev, out in pairs:
-            for t, name in ((prev, "d_prev"), (out, "d_out")):
-                if t is None:
-                    if name == "d_out" or self.coeffs[4] != 0.0:
-                        raise _lib.RttiError(f"multistep blend: {name} is required")
-                    continue
-                _req(t, torch.float32, name)
-                if not t.is_contiguous() or t.numel() != n:
-                    raise _lib.RttiError(f"multistep blend: {name} must be a contiguous fp32 tensor of {n} elements")
-
-    def args(self, ref=False):
-        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(self.d_prev), _ptr(self.d_out)]
-        return a + ([_ptr(self.d_prev_ref), _ptr(self.d_out_ref)] if ref else [])
+    def _needed(self):
+        return self.coeffs[4] != 0.0, True
 
 
-class AncestralStep:
+class AncestralStep(_Step):
     """The Euler Ancestral update of one blend call: x' = x + dt eps + s_up z, with (dt, s_up) from
     schedulers.EulerAncestralDiscreteScheduler.ancestral_coeffs and z the fp16 noise of the step, [n] elements (read only
     when s_up != 0). z_ref: the reference-latent trajectory's noise (gather_blend_step only); both trajectories take the
     same dt and s_up."""
+    form, what, names, dtypes = "_anc", "ancestral", ("z",), (_F16,)
 
     def __init__(self, dt, s_up, z, z_ref=None):
-        self.dt, self.s_up = float(dt), float(s_up)
-        self.z, self.z_ref = z, z_ref
+        super().__init__((dt, s_up), (z,), (z_ref,))
 
-    def _check(self, n, ref):
-        for t, name in [(self.z, "z")] + ([(self.z_ref, "z_ref")] if ref else []):
-            if t is None:
-                if self.s_up != 0.0:
-                    raise _lib.RttiError(f"ancestral blend: {name} is required")
-                continue
-            _req(t, _F16, name)
-            if not t.is_contiguous() or t.numel() != n:
-                raise _lib.RttiError(f"ancestral blend: {name} must be a contiguous fp16 tensor of {n} elements")
-
-    def args(self, ref=False):
-        a = [ctypes.c_float(self.dt), ctypes.c_float(self.s_up), _ptr(self.z)]
-        return a + ([_ptr(self.z_ref)] if ref else [])
+    def _needed(self):
+        return (self.coeffs[1] != 0.0,)
 
 
 class UniPCHistory:
@@ -283,157 +332,77 @@ class UniPCHistory:
         self.m1, self.m2 = self.m2, self.m1
 
 
-class UniPCStep:
+class UniPCStep(_Step):
     """The UniPC update of one blend call: `coeffs` (schedulers.UniPCCoeffs) and the fp32 [n] buffers of one trajectory,
     (xl, m1, m2, m_out, xl_out): xl read when ul != 0, m1 when u1 or v1 != 0, m2 when u2 != 0; m_out (may be m2) and
     xl_out (may be xl) written. `ref`: the same five buffers of the reference-latent trajectory (gather_blend_step only).
     `UniPCStep.of(coeffs, hist, hist_ref)` steps UniPCHistory objects in place (call their rotate() afterwards)."""
+    form, what = "_unipc", "UniPC"
+    names, dtypes = ("xl", "m1", "m2", "m_out", "xl_out"), (torch.float32,) * 5
 
     def __init__(self, coeffs, xl, m1, m2, m_out, xl_out, ref=None):
-        self.coeffs = tuple(float(c) for c in coeffs)
-        self.bufs = (xl, m1, m2, m_out, xl_out)
-        self.ref = tuple(ref) if ref is not None else None
+        super().__init__(coeffs, (xl, m1, m2, m_out, xl_out), ref)
 
     @classmethod
     def of(cls, coeffs, hist, hist_ref=None):
         b = lambda h: (h.xl, h.m1, h.m2, h.m2, h.xl)
         return cls(coeffs, *b(hist), ref=b(hist_ref) if hist_ref is not None else None)
 
-    def _check(self, n, ref):
+    def _needed(self):
         _, _, _, ul, _, u1, u2, _, _, v1 = self.coeffs
-        needed = (ul != 0.0, u1 != 0.0 or v1 != 0.0, u2 != 0.0, True, True)
-        names = ("xl", "m1", "m2", "m_out", "xl_out")
-        sets = [self.bufs] + ([self.ref or (None,) * 5] if ref else [])
-        for bufs in sets:
-            for t, need, name in zip(bufs, needed, names):
-                if t is None:
-                    if need:
-                        raise _lib.RttiError(f"UniPC blend: {name} is required")
-                    continue
-                _req(t, torch.float32, name)
-                if not t.is_contiguous() or t.numel() != n:
-                    raise _lib.RttiError(f"UniPC blend: {name} must be a contiguous fp32 tensor of {n} elements")
-
-    def args(self, ref=False):
-        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(t) for t in self.bufs]
-        return a + ([_ptr(t) for t in (self.ref or (None,) * 5)] if ref else [])
+        return ul != 0.0, u1 != 0.0 or v1 != 0.0, u2 != 0.0, True, True
 
 
-class HeunStep:
+class HeunStep(_Step):
     """The Heun update of one blend call: `coeffs` (cx, ce, cs, cd) from schedulers.HeunDiscreteScheduler.heun_coeffs,
     x' = cx x + ce eps + cs xs + cd ds, with xs / ds the fp16 [n] latents and stepped noise prediction saved at the last
     first stage (xs read when cs != 0, ds when cd != 0; may be None otherwise). xs_ref / ds_ref: the reference-latent
     trajectory's; eps_ref_out: an fp16 [n] tensor that receives that trajectory's stepped prediction, or None
     (gather_blend_step only)."""
+    form, what, names, dtypes, coeff_names = "_heun", "Heun", ("xs", "ds"), (_F16,) * 2, ("cx", "ce", "cs", "cd")
+    has_eps_ref_out = True
 
     def __init__(self, coeffs, xs, ds, xs_ref=None, ds_ref=None, eps_ref_out=None):
-        self.coeffs = tuple(float(c) for c in coeffs)
-        if len(self.coeffs) != 4:
-            raise _lib.RttiError(f"Heun blend: coeffs must be (cx, ce, cs, cd), got {len(self.coeffs)} values")
-        self.xs, self.ds, self.xs_ref, self.ds_ref, self.eps_ref_out = xs, ds, xs_ref, ds_ref, eps_ref_out
+        super().__init__(coeffs, (xs, ds), (xs_ref, ds_ref), eps_ref_out)
 
-    def _check(self, n, ref):
-        _, _, cs, cd = self.coeffs
-        items = [(self.xs, cs != 0.0, "xs"), (self.ds, cd != 0.0, "ds")]
-        if ref:
-            items += [(self.xs_ref, cs != 0.0, "xs_ref"), (self.ds_ref, cd != 0.0, "ds_ref"),
-                      (self.eps_ref_out, False, "eps_ref_out")]
-        elif self.eps_ref_out is not None:
-            raise _lib.RttiError("Heun blend: eps_ref_out needs the reference latents")
-        for t, need, name in items:
-            if t is None:
-                if need:
-                    raise _lib.RttiError(f"Heun blend: {name} is required")
-                continue
-            _req(t, _F16, name)
-            if not t.is_contiguous() or t.numel() != n:
-                raise _lib.RttiError(f"Heun blend: {name} must be a contiguous fp16 tensor of {n} elements")
-
-    def args(self, ref=False):
-        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(self.xs), _ptr(self.ds)]
-        return a + ([_ptr(self.xs_ref), _ptr(self.ds_ref), _ptr(self.eps_ref_out)] if ref else [])
+    def _needed(self):
+        return self.coeffs[2] != 0.0, self.coeffs[3] != 0.0
 
 
-def _overlap(a, b):
-    """Whether the storage spans of two tensors intersect."""
-    a0, b0 = a.data_ptr(), b.data_ptr()
-    return a0 < b0 + b.numel() * b.element_size() and b0 < a0 + a.numel() * a.element_size()
-
-
-class LMSStep:
+class LMSStep(_Step):
     """The LMS update of one blend call: `coeffs` (c0, c1, c2, c3) from schedulers.LMSDiscreteScheduler.lms_coeffs,
     x' = x + c0 eps + c1 d1 + c2 d2 + c3 d3, with d1, d2, d3 the fp16 [n] stepped noise predictions of the trajectory's
     last three steps, newest first (d_k read when c_k != 0; may be None otherwise). d1_ref / d2_ref / d3_ref: the
     reference-latent trajectory's; eps_ref_out: an fp16 [n] tensor that receives that trajectory's stepped prediction,
     or None (gather_blend_step only). The histories are only read; no output may overlap them."""
+    form, what, names, dtypes, coeff_names = "_lms", "LMS", ("d1", "d2", "d3"), (_F16,) * 3, ("c0", "c1", "c2", "c3")
+    read_only, has_eps_ref_out = names, True
 
     def __init__(self, coeffs, d1, d2, d3, d1_ref=None, d2_ref=None, d3_ref=None, eps_ref_out=None):
-        self.coeffs = tuple(float(c) for c in coeffs)
-        if len(self.coeffs) != 4:
-            raise _lib.RttiError(f"LMS blend: coeffs must be (c0, c1, c2, c3), got {len(self.coeffs)} values")
-        self.d, self.d_ref, self.eps_ref_out = (d1, d2, d3), (d1_ref, d2_ref, d3_ref), eps_ref_out
+        super().__init__(coeffs, (d1, d2, d3), (d1_ref, d2_ref, d3_ref), eps_ref_out)
 
-    def _check(self, n, ref, outs=()):
-        """`outs`: the output tensors of the call, which must not overlap a history."""
-        c = self.coeffs[1:]
-        items = [(t, ck != 0.0, f"d{k + 1}") for k, (t, ck) in enumerate(zip(self.d, c))]
-        if ref:
-            items += [(t, ck != 0.0, f"d{k + 1}_ref") for k, (t, ck) in enumerate(zip(self.d_ref, c))]
-            items.append((self.eps_ref_out, False, "eps_ref_out"))
-        elif self.eps_ref_out is not None:
-            raise _lib.RttiError("LMS blend: eps_ref_out needs the reference latents")
-        for t, need, name in items:
-            if t is None:
-                if need:
-                    raise _lib.RttiError(f"LMS blend: {name} is required")
-                continue
-            _req(t, _F16, name)
-            if not t.is_contiguous() or t.numel() != n:
-                raise _lib.RttiError(f"LMS blend: {name} must be a contiguous fp16 tensor of {n} elements")
-        outs = [o for o in outs if o is not None] + ([self.eps_ref_out] if ref and self.eps_ref_out is not None else [])
-        for t, _, name in items:
-            if t is not None and name != "eps_ref_out" and any(_overlap(t, o) for o in outs):
-                raise _lib.RttiError(f"LMS blend: {name} overlaps an output of the call")
-
-    def args(self, ref=False):
-        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(t) for t in self.d]
-        return a + ([_ptr(t) for t in self.d_ref] + [_ptr(self.eps_ref_out)] if ref else [])
+    def _needed(self):
+        return tuple(c != 0.0 for c in self.coeffs[1:])
 
 
-class SinglestepStep:
+class SinglestepStep(_Step):
     """The DPM-Solver++(2S) update of one blend call: `coeffs` (schedulers.SinglestepCoeffs: hx, he, cx, cs, cd, cp),
     D = hx x + he eps, x' = cx x + cd D + cp D_prev + cs xs. d_prev / d_out: the fp32 [n] D buffers as in MultistepStep
     (d_prev read when cp != 0, may be the same tensor as d_out); xs: the fp16 [n] latents that entered the block's first
     step (read when cs != 0; may be None otherwise; only read, so no output may overlap it). d_prev_ref / d_out_ref /
     xs_ref: the reference-latent trajectory's (gather_blend_step only)."""
+    form, what, coeff_names = "_ss", "singlestep", ("hx", "he", "cx", "cs", "cd", "cp")
+    names, dtypes, read_only = ("d_prev", "d_out", "xs"), (torch.float32, torch.float32, _F16), ("xs",)
 
     def __init__(self, coeffs, d_prev, d_out, xs, d_prev_ref=None, d_out_ref=None, xs_ref=None):
-        self.coeffs = tuple(float(c) for c in coeffs)
-        if len(self.coeffs) != 6:
-            raise _lib.RttiError(f"singlestep blend: coeffs must be (hx, he, cx, cs, cd, cp), got {len(self.coeffs)} values")
-        self.main, self.ref = (d_prev, d_out, xs), (d_prev_ref, d_out_ref, xs_ref)
+        super().__init__(coeffs, (d_prev, d_out, xs), (d_prev_ref, d_out_ref, xs_ref))
 
-    def _check(self, n, ref, outs=()):
-        """`outs`: the fp16 output tensors of the call, which must not overlap xs."""
-        _, _, _, cs, _, cp = self.coeffs
-        outs = [o for o in outs if o is not None]
-        for (d_prev, d_out, xs), sfx in [(self.main, "")] + ([(self.ref, "_ref")] if ref else []):
-            for t, need, dtype, name in ((d_prev, cp != 0.0, torch.float32, "d_prev"), (d_out, True, torch.float32, "d_out"),
-                                         (xs, cs != 0.0, _F16, "xs")):
-                if t is None:
-                    if need:
-                        raise _lib.RttiError(f"singlestep blend: {name}{sfx} is required")
-                    continue
-                _req(t, dtype, name + sfx)
-                if not t.is_contiguous() or t.numel() != n:
-                    raise _lib.RttiError(f"singlestep blend: {name}{sfx} must be a contiguous {dtype} tensor of {n} "
-                                         "elements")
-            if xs is not None and any(_overlap(xs, o) for o in outs):
-                raise _lib.RttiError(f"singlestep blend: xs{sfx} overlaps an output of the call")
+    def _needed(self):
+        return self.coeffs[5] != 0.0, True, self.coeffs[3] != 0.0
 
-    def args(self, ref=False):
-        a = [ctypes.c_float(c) for c in self.coeffs] + [_ptr(t) for t in self.main]
-        return a + ([_ptr(t) for t in self.ref] if ref else [])
+
+def _blend_symbol(base, guidance_rescale, step):
+    return f"rtti_{base}{'_rescale' if guidance_rescale != 0.0 else ''}{step.form}"
 
 
 def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_sigma=0.0, guidance_rescale=0.0,
@@ -441,16 +410,11 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     """eps = eps_u + g (eps_t - eps_u) with the masked region sums; optionally latents + dt_sigma*eps.
     eps_regions: list of fp16 tensors (region passes in mask order, base-prompt pass last); masks fp32 [N, n].
     guidance_rescale = phi > 0 scales eps by 1 - phi + phi std(eps_t) / std(eps) before it is stored and stepped
-    (rtti_region_blend_cfg_rescale); phi == 0 runs rtti_region_blend_cfg.
-    step: a MultistepStep — the latents (required then) take the DDIM / DPM-Solver++ update instead of the Euler one
-    (rtti_region_blend_cfg_ms / rtti_region_blend_cfg_rescale_ms; dt_sigma is not used); an AncestralStep — the
-    Euler Ancestral update (rtti_region_blend_cfg_anc / rtti_region_blend_cfg_rescale_anc; dt_sigma is not used); a
-    UniPCStep — the UniPC update (rtti_region_blend_cfg_unipc / rtti_region_blend_cfg_rescale_unipc; dt_sigma is not
-    used); a HeunStep — the Heun update (rtti_region_blend_cfg_heun / rtti_region_blend_cfg_rescale_heun; dt_sigma is
-    not used, nor are xs_ref / ds_ref; eps_ref_out must be None); an LMSStep — the LMS update (rtti_region_blend_cfg_lms
-    / rtti_region_blend_cfg_rescale_lms; dt_sigma is not used, nor are d1_ref / d2_ref / d3_ref; eps_ref_out must be
-    None); a SinglestepStep — the DPM-Solver++(2S) update (rtti_region_blend_cfg_ss / rtti_region_blend_cfg_rescale_ss;
-    dt_sigma is not used, nor are the _ref buffers)."""
+    (rtti_region_blend_cfg_rescale*); phi == 0 runs rtti_region_blend_cfg*.
+    step: the scheduler update of the latents (required then), one of EulerStep (dt_sigma is shorthand for
+    EulerStep(dt_sigma)), MultistepStep, AncestralStep, UniPCStep, HeunStep, LMSStep or SinglestepStep; it selects the
+    entry point by its form (rtti_region_blend_cfg_ms, ..._anc, ..._unipc, ..._heun, ..._lms, ..._ss). The buffers of
+    the reference trajectory are not used here; eps_ref_out must be None."""
     lib = _lib.load()
     _req(eps_uncond, _F16, "eps_uncond"); _req(masks, torch.float32, "masks")
     n = eps_uncond.numel()
@@ -458,96 +422,19 @@ def region_blend_cfg(eps_uncond, eps_regions, masks, guidance, latents=None, dt_
     assert masks.is_contiguous() and masks.numel() == N * n
     for e in eps_regions:
         _req(e, _F16, "eps_region"); assert e.is_contiguous() and e.numel() == n
+    if step is None:
+        step = EulerStep(dt_sigma)
+    elif latents is None:
+        raise _lib.RttiError(f"region_blend_cfg: a {type(step).__name__} needs the latents")
     ptrs = (ctypes.c_void_p * N)(*[e.data_ptr() for e in eps_regions])
     eps_out = torch.empty_like(eps_uncond)
     lat_out = torch.empty_like(latents) if latents is not None else None
-    if isinstance(step, SinglestepStep):
-        if latents is None:
-            raise _lib.RttiError("region_blend_cfg: a singlestep step needs the latents")
-        step._check(n, False, (eps_out, lat_out))
-        if guidance_rescale == 0.0:
-            rc = lib.rtti_region_blend_cfg_ss(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                              _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_ss")
-        else:
-            rc = lib.rtti_region_blend_cfg_rescale_ss(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                      _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
-                                                      float(guidance_rescale), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_rescale_ss")
-    elif isinstance(step, LMSStep):
-        if latents is None:
-            raise _lib.RttiError("region_blend_cfg: an LMS step needs the latents")
-        step._check(n, False, (eps_out, lat_out))
-        if guidance_rescale == 0.0:
-            rc = lib.rtti_region_blend_cfg_lms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                               _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_lms")
-        else:
-            rc = lib.rtti_region_blend_cfg_rescale_lms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                       _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
-                                                       float(guidance_rescale), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_rescale_lms")
-    elif isinstance(step, HeunStep):
-        if latents is None:
-            raise _lib.RttiError("region_blend_cfg: a Heun step needs the latents")
-        step._check(n, False)
-        if guidance_rescale == 0.0:
-            rc = lib.rtti_region_blend_cfg_heun(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_heun")
-        else:
-            rc = lib.rtti_region_blend_cfg_rescale_heun(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                        _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
-                                                        float(guidance_rescale), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_rescale_heun")
-    elif isinstance(step, UniPCStep):
-        if latents is None:
-            raise _lib.RttiError("region_blend_cfg: a UniPC step needs the latents")
-        step._check(n, False)
-        if guidance_rescale == 0.0:
-            rc = lib.rtti_region_blend_cfg_unipc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                 _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_unipc")
-        else:
-            rc = lib.rtti_region_blend_cfg_rescale_unipc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                         _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
-                                                         float(guidance_rescale), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_rescale_unipc")
-    elif isinstance(step, AncestralStep):
-        if latents is None:
-            raise _lib.RttiError("region_blend_cfg: an ancestral step needs the latents")
-        step._check(n, False)
-        if guidance_rescale == 0.0:
-            rc = lib.rtti_region_blend_cfg_anc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
-                                               _ptr(latents), _ptr(lat_out), *step.args(), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_anc")
-        else:
-            rc = lib.rtti_region_blend_cfg_rescale_anc(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                       _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
-                                                       float(guidance_rescale), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_rescale_anc")
-    elif step is not None:
-        if latents is None:
-            raise _lib.RttiError("region_blend_cfg: a multistep step needs the latents")
-        step._check(n, False)
-        if guidance_rescale == 0.0:
-            rc = lib.rtti_region_blend_cfg_ms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
-                                              _ptr(latents), _ptr(lat_out), *step.args(), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_ms")
-        else:
-            rc = lib.rtti_region_blend_cfg_rescale_ms(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance),
-                                                      _ptr(eps_out), _ptr(latents), _ptr(lat_out), *step.args(),
-                                                      float(guidance_rescale), _stream())
-            _lib.check(rc, "rtti_region_blend_cfg_rescale_ms")
-    elif guidance_rescale == 0.0:
-        rc = lib.rtti_region_blend_cfg(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
-                                       _ptr(latents), _ptr(lat_out), float(dt_sigma), _stream())
-        _lib.check(rc, "rtti_region_blend_cfg")
-    else:
-        rc = lib.rtti_region_blend_cfg_rescale(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out),
-                                               _ptr(latents), _ptr(lat_out), float(dt_sigma), float(guidance_rescale),
-                                               _stream())
-        _lib.check(rc, "rtti_region_blend_cfg_rescale")
+    step._check(n, False, (eps_out, lat_out))
+    symbol = _blend_symbol("region_blend_cfg", guidance_rescale, step)
+    phi = [float(guidance_rescale)] if guidance_rescale != 0.0 else []
+    rc = getattr(lib, symbol)(_ptr(eps_uncond), ptrs, _ptr(masks), N, n, float(guidance), _ptr(eps_out), _ptr(latents),
+                              _ptr(lat_out), *step.args(), *phi, _stream())
+    _lib.check(rc, symbol)
     _count(1)
     return (eps_out, lat_out) if latents is not None else eps_out
 
@@ -617,99 +504,29 @@ def predict_x0(x_t, eps, alpha):
 
 def gather_blend_step(peer_slot_ptrs, peer_flag_ptrs, rank, slot_owner, n_regions, masks, guidance, latents, latents_ref,
                       dt_sigma, step_id, guidance_rescale=0.0, step=None):
-    """Fused all-gather + blend + CFG + Euler over NVLink peer memory (rtti_gather_blend_step; with
-    guidance_rescale > 0 rtti_gather_blend_step_rescale, which also rescales the reference-latent pair).
-    step: a MultistepStep (with d_prev_ref / d_out_ref when latents_ref is given) — the DDIM / DPM-Solver++ update
-    instead of the Euler one (rtti_gather_blend_step_ms / rtti_gather_blend_step_rescale_ms); an AncestralStep (with
-    z_ref when latents_ref is given) — the Euler Ancestral update (rtti_gather_blend_step_anc /
-    rtti_gather_blend_step_rescale_anc); a UniPCStep (with `ref` when latents_ref is given) — the UniPC update
-    (rtti_gather_blend_step_unipc / rtti_gather_blend_step_rescale_unipc); a HeunStep (with xs_ref / ds_ref, and
-    optionally eps_ref_out, when latents_ref is given) — the Heun update (rtti_gather_blend_step_heun /
-    rtti_gather_blend_step_rescale_heun); an LMSStep (with d1_ref / d2_ref / d3_ref, and optionally eps_ref_out, when
-    latents_ref is given) — the LMS update (rtti_gather_blend_step_lms / rtti_gather_blend_step_rescale_lms); a
-    SinglestepStep (with d_prev_ref / d_out_ref / xs_ref when latents_ref is given) — the DPM-Solver++(2S) update
-    (rtti_gather_blend_step_ss / rtti_gather_blend_step_rescale_ss).
+    """Fused all-gather + blend + CFG + scheduler update over NVLink peer memory (rtti_gather_blend_step*; with
+    guidance_rescale > 0 the _rescale entry points, which also rescale the reference-latent pair).
+    step: as for region_blend_cfg (None: EulerStep(dt_sigma)), with the reference trajectory's buffers (and, for Heun
+    and LMS, optionally eps_ref_out) when latents_ref is given.
     Returns (eps, latents_out, latents_ref_out or None)."""
     lib = _lib.load()
     world = len(peer_slot_ptrs)
     n = latents.numel()
     _req(latents, _F16, "latents"); _req(masks, torch.float32, "masks")
+    if step is None:
+        step = EulerStep(dt_sigma)
     eps = torch.empty_like(latents)
     lat_out = torch.empty_like(latents)
     ref_out = torch.empty_like(latents_ref) if latents_ref is not None else None
+    step._check(n, latents_ref is not None, (eps, lat_out, ref_out))
     slots = (ctypes.c_void_p * world)(*peer_slot_ptrs)
     flags = (ctypes.c_void_p * world)(*peer_flag_ptrs)
-    if isinstance(step, SinglestepStep):
-        step._check(n, latents_ref is not None, (eps, lat_out, ref_out))
-        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
-                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
-        args += step.args(ref=True) + [int(step_id)]
-        if guidance_rescale == 0.0:
-            _lib.check(lib.rtti_gather_blend_step_ss(*args, _stream()), "rtti_gather_blend_step_ss")
-        else:
-            _lib.check(lib.rtti_gather_blend_step_rescale_ss(*args, float(guidance_rescale), _stream()),
-                       "rtti_gather_blend_step_rescale_ss")
-    elif isinstance(step, LMSStep):
-        step._check(n, latents_ref is not None, (eps, lat_out, ref_out))
-        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
-                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
-        args += step.args(ref=True) + [int(step_id)]
-        if guidance_rescale == 0.0:
-            _lib.check(lib.rtti_gather_blend_step_lms(*args, _stream()), "rtti_gather_blend_step_lms")
-        else:
-            _lib.check(lib.rtti_gather_blend_step_rescale_lms(*args, float(guidance_rescale), _stream()),
-                       "rtti_gather_blend_step_rescale_lms")
-    elif isinstance(step, HeunStep):
-        step._check(n, latents_ref is not None)
-        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
-                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
-        args += step.args(ref=True) + [int(step_id)]
-        if guidance_rescale == 0.0:
-            _lib.check(lib.rtti_gather_blend_step_heun(*args, _stream()), "rtti_gather_blend_step_heun")
-        else:
-            _lib.check(lib.rtti_gather_blend_step_rescale_heun(*args, float(guidance_rescale), _stream()),
-                       "rtti_gather_blend_step_rescale_heun")
-    elif isinstance(step, UniPCStep):
-        step._check(n, latents_ref is not None)
-        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
-                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
-        args += step.args(ref=True) + [int(step_id)]
-        if guidance_rescale == 0.0:
-            _lib.check(lib.rtti_gather_blend_step_unipc(*args, _stream()), "rtti_gather_blend_step_unipc")
-        else:
-            _lib.check(lib.rtti_gather_blend_step_rescale_unipc(*args, float(guidance_rescale), _stream()),
-                       "rtti_gather_blend_step_rescale_unipc")
-    elif isinstance(step, AncestralStep):
-        step._check(n, latents_ref is not None)
-        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
-                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
-        args += step.args(ref=True) + [int(step_id)]
-        if guidance_rescale == 0.0:
-            _lib.check(lib.rtti_gather_blend_step_anc(*args, _stream()), "rtti_gather_blend_step_anc")
-        else:
-            _lib.check(lib.rtti_gather_blend_step_rescale_anc(*args, float(guidance_rescale), _stream()),
-                       "rtti_gather_blend_step_rescale_anc")
-    elif step is not None:
-        step._check(n, latents_ref is not None)
-        args = [slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks), n,
-                float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out)]
-        args += step.args(ref=True) + [int(step_id)]
-        if guidance_rescale == 0.0:
-            _lib.check(lib.rtti_gather_blend_step_ms(*args, _stream()), "rtti_gather_blend_step_ms")
-        else:
-            _lib.check(lib.rtti_gather_blend_step_rescale_ms(*args, float(guidance_rescale), _stream()),
-                       "rtti_gather_blend_step_rescale_ms")
-    elif guidance_rescale == 0.0:
-        rc = lib.rtti_gather_blend_step(slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions,
-                                        _ptr(masks), n, float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out),
-                                        _ptr(latents_ref), _ptr(ref_out), float(dt_sigma), int(step_id), _stream())
-        _lib.check(rc, "rtti_gather_blend_step")
-    else:
-        rc = lib.rtti_gather_blend_step_rescale(slots, flags, world, rank, _int_array(slot_owner), len(slot_owner),
-                                                n_regions, _ptr(masks), n, float(guidance), _ptr(eps), _ptr(latents),
-                                                _ptr(lat_out), _ptr(latents_ref), _ptr(ref_out), float(dt_sigma),
-                                                int(step_id), float(guidance_rescale), _stream())
-        _lib.check(rc, "rtti_gather_blend_step_rescale")
+    symbol = _blend_symbol("gather_blend_step", guidance_rescale, step)
+    phi = [float(guidance_rescale)] if guidance_rescale != 0.0 else []
+    rc = getattr(lib, symbol)(slots, flags, world, rank, _int_array(slot_owner), len(slot_owner), n_regions, _ptr(masks),
+                              n, float(guidance), _ptr(eps), _ptr(latents), _ptr(lat_out), _ptr(latents_ref),
+                              _ptr(ref_out), *step.args(ref=True), int(step_id), *phi, _stream())
+    _lib.check(rc, symbol)
     _count(1)
     return eps, lat_out, ref_out
 

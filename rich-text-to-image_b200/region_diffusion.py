@@ -7,12 +7,9 @@ models/region_diffusion.py:86-174 (including its differences from the SDXL loop:
 joint stepping on every step when injecting, `i == int(...)` background flag, and the self-attention
 capture that overwrites instead of accumulating, :423), executed as one batched UNet call per step.
 
-`.scheduler` is PLMS (PNDMScheduler) by default and steps on the host; DDIMScheduler and DPMSolverMultistepScheduler
-(schedulers.py) step inside the fused blend kernels (rtti_region_blend_cfg_ms), with one fp32 history of the x0
-prediction per trajectory; UniPCMultistepScheduler steps inside rtti_region_blend_cfg_unipc, with three fp32 histories
-per trajectory (ops.UniPCHistory); DPMSolverSinglestepScheduler (DPM-Solver++(2S)) steps inside
-rtti_region_blend_cfg_ss, with one fp32 history of the x0 prediction and the fp16 latents that entered the current
-two-step block per trajectory.
+`.scheduler` is PLMS (PNDMScheduler) by default and steps on the host; DDIMScheduler, DPMSolverMultistepScheduler,
+UniPCMultistepScheduler and DPMSolverSinglestepScheduler (schedulers.py) step inside the fused blend kernels, with
+their state kept per trajectory (stepping.py).
 """
 import math
 from typing import Optional
@@ -20,12 +17,16 @@ from typing import Optional
 import numpy as np
 import torch
 
-from . import ops, region_parallel, vae_guidance
+from . import ops, region_parallel, stepping, vae_guidance
 from .attention_utils import CrossAttentionLayers, SelfAttentionLayers
 from .lora import LoraLoaderMixin
-from .schedulers import MULTISTEP_SCHEDULERS, DPMSolverSinglestepScheduler, PNDMScheduler, UniPCMultistepScheduler
+from .schedulers import PNDMScheduler
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
+
+
+# the updates that run fused here; any other scheduler steps on the host, on the concatenated batch
+_FUSED = ("multistep", "unipc", "singlestep")
 
 
 class RegionDiffusion(LoraLoaderMixin):
@@ -150,16 +151,9 @@ class RegionDiffusion(LoraLoaderMixin):
             word_pos = font_size = None
         kv_caches = {}
         n_t = len(timesteps)
-        multistep = isinstance(self.scheduler, MULTISTEP_SCHEDULERS)
-        singlestep = isinstance(self.scheduler, DPMSolverSinglestepScheduler)
-        xs = xs_ref = None   # 2S: the latents that entered the current block's first step, per trajectory
-        if multistep or singlestep:   # one x0-prediction history per trajectory (both are stepped on every step)
-            d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev)
-            d_hist_ref = torch.empty_like(d_hist) if inject else None
-        unipc = isinstance(self.scheduler, UniPCMultistepScheduler)
-        if unipc:       # one UniPC state per trajectory (both are stepped on every step)
-            up_hist = ops.UniPCHistory(latents.numel(), dev)
-            up_hist_ref = ops.UniPCHistory(latents.numel(), dev) if inject else None
+        stepper = stepping.stepper(self.scheduler, latents.shape, dev, kinds=_FUSED)
+        if stepper is not None:   # both trajectories are stepped on every step
+            main, ref = stepper.state(), (stepper.state() if inject else None)
         for i, t in enumerate(timesteps):
             feat_inject_step = bool(int(t) > (1 - inject_selfattn) * 1000)                                   # :104
             background_inject_step = (i == int(inject_background * n_t)) and inject_background > 0           # :105
@@ -179,41 +173,19 @@ class RegionDiffusion(LoraLoaderMixin):
             eps = plan.gather(eps_local, local, feat_inject_step)
             regions = [eps[kind[f"E{j}"]:kind[f"E{j}"] + 1].contiguous() for j in range(N - 1)]
             regions.append(eps[kind["B"]:kind["B"] + 1].contiguous())
-            if multistep:
-                c = self.scheduler.step_coeffs(i)
+            if stepper is not None:
+                stepper.begin(i, t, 2 if inject else 1)
+                lat = latents.contiguous()
                 noise_pred, latents = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks,
-                                                           guidance_scale, latents=latents.contiguous(),
-                                                           step=ops.MultistepStep(c, d_hist, d_hist))
+                                                           guidance_scale, latents=lat, step=stepper.step(main))
+                main = stepper.advance(main, lat, noise_pred)
                 if inject:
-                    _, latents_ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
-                                                          [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale,
-                                                          latents=latents_ref.contiguous(),
-                                                          step=ops.MultistepStep(c, d_hist_ref, d_hist_ref))
-            elif unipc:
-                c = self.scheduler.unipc_coeffs(i)
-                noise_pred, latents = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks,
-                                                           guidance_scale, latents=latents.contiguous(),
-                                                           step=ops.UniPCStep.of(c, up_hist))
-                up_hist.rotate()
-                if inject:
-                    _, latents_ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
-                                                          [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale,
-                                                          latents=latents_ref.contiguous(),
-                                                          step=ops.UniPCStep.of(c, up_hist_ref))
-                    up_hist_ref.rotate()
-            elif singlestep:
-                c = self.scheduler.singlestep_coeffs(i)
-                lat, lat_ref = latents.contiguous(), (latents_ref.contiguous() if inject else None)
-                noise_pred, latents = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks,
-                                                           guidance_scale, latents=lat,
-                                                           step=ops.SinglestepStep(c, d_hist, d_hist, xs))
-                if inject:
-                    _, latents_ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
-                                                          [eps[kind["D"]:kind["D"] + 1].contiguous()], ones, guidance_scale,
-                                                          latents=lat_ref,
-                                                          step=ops.SinglestepStep(c, d_hist_ref, d_hist_ref, xs_ref))
-                if self.scheduler.is_first_step(i):
-                    xs, xs_ref = lat, lat_ref
+                    lat_ref = latents_ref.contiguous()
+                    eps_ref, latents_ref = ops.region_blend_cfg(eps[kind["C"]:kind["C"] + 1].contiguous(),
+                                                                [eps[kind["D"]:kind["D"] + 1].contiguous()], ones,
+                                                                guidance_scale, latents=lat_ref,
+                                                                step=stepper.step(ref, 1))
+                    ref = stepper.advance(ref, lat_ref, eps_ref)
             else:
                 noise_pred = ops.region_blend_cfg(eps[kind["A"]:kind["A"] + 1].contiguous(), regions, masks, guidance_scale)  # :119-132
                 if inject:                                                                                  # :134-143
@@ -245,33 +217,18 @@ class RegionDiffusion(LoraLoaderMixin):
         self.scheduler.set_timesteps(num_inference_steps)
         kv = CrossKVCache()
         ones = torch.ones(1, latents[0].numel(), dtype=torch.float32, device=dev)
-        multistep = isinstance(self.scheduler, MULTISTEP_SCHEDULERS)
-        singlestep = isinstance(self.scheduler, DPMSolverSinglestepScheduler)
-        d_hist = torch.empty(latents.numel(), dtype=torch.float32, device=dev) if multistep or singlestep else None
-        xs = None   # 2S: the latents that entered the current block's first step
-        up_hist = ops.UniPCHistory(latents.numel(), dev) if isinstance(self.scheduler, UniPCMultistepScheduler) else None
+        stepper = stepping.stepper(self.scheduler, latents.shape, dev, kinds=_FUSED)
+        state = stepper.state() if stepper is not None else None
         for i, t in enumerate(self.scheduler.timesteps):
             x = latents.expand(2, -1, -1, -1)
             ctrl = RegionControl(capture=self._capture, capture_row=1, kv_cache=kv)
             eps = self.unet(x, t, ctx, None, ctrl)["sample"]
-            if multistep:
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=latents.contiguous(),
-                                                  step=ops.MultistepStep(self.scheduler.step_coeffs(i), d_hist, d_hist))
-                continue
-            if up_hist is not None:
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=latents.contiguous(),
-                                                  step=ops.UniPCStep.of(self.scheduler.unipc_coeffs(i), up_hist))
-                up_hist.rotate()
-                continue
-            if singlestep:
+            if stepper is not None:
+                stepper.begin(i, t, 1)
                 lat = latents.contiguous()
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=lat, step=ops.SinglestepStep(
-                                                      self.scheduler.singlestep_coeffs(i), d_hist, d_hist, xs))
-                if self.scheduler.is_first_step(i):
-                    xs = lat
+                e16, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                    latents=lat, step=stepper.step(state))
+                state = stepper.advance(state, lat, e16)
                 continue
             noise_pred = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale)
             latents = self.scheduler.step(noise_pred, t, latents)["prev_sample"].to(torch.float16)

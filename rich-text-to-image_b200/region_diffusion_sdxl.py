@@ -8,12 +8,7 @@ semantics (models/region_diffusion_sdxl.py:772-914), re-organised for the hardwa
     base, N-1 regions; :787-821) run as ONE batched UNet call — they share the timestep and, up to the
     reference latent, the input; the hook choreography becomes a RegionControl;
   * region blend + CFG (+ guidance rescale) + scheduler update is one kernel (rtti_region_blend_cfg, or
-    rtti_region_blend_cfg_rescale with guidance_rescale > 0; their "_ms" forms for DDIM / DPM-Solver++(2M), which
-    keep one fp32 history of the x0 prediction per trajectory, "_anc" forms for Euler Ancestral, which add the
-    noise drawn for the step, "_unipc" forms for UniPC, which keep three fp32 histories per trajectory, "_heun"
-    forms for Heun's method, which read the fp16 latents and prediction saved at the first stage, "_lms" forms for
-    k-LMS, which read the fp16 predictions of the last three steps, and "_ss" forms for DPM-Solver++(2S), which keep
-    one fp32 history of the x0 prediction per trajectory and read the fp16 latents that entered the two-step block);
+    rtti_region_blend_cfg_rescale with guidance_rescale > 0, in the form of the scheduler's update: stepping.py);
     colour-guidance loss fwd/bwd,
     guidance update, x0 prediction and background injection are kernels too;
   * with torch.distributed initialised the passes are sharded over the ranks (region_parallel.py) and the
@@ -25,11 +20,11 @@ from typing import List, Optional
 import numpy as np
 import torch
 
-from . import ops, region_parallel, vae_guidance
+from . import ops, region_parallel, stepping, vae_guidance
 from .attention_utils import CrossAttentionLayers_XL
 from .lora import LoraLoaderMixin
-from .schedulers import (MULTISTEP_SCHEDULERS, DDIMScheduler, DPMSolverSinglestepScheduler, EulerAncestralDiscreteScheduler,
-                         EulerDiscreteScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler, UniPCMultistepScheduler)
+from .schedulers import DDIMScheduler, EulerDiscreteScheduler
+from .stepping import _step_kind  # noqa: F401  (re-exported)
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -37,32 +32,6 @@ from .vae import AutoencoderKLDecoder, VAEConfig
 def _rescale_phi(guidance_scale, guidance_rescale):
     """The guidance rescale in effect: the reference applies it only with classifier-free guidance on (:903)."""
     return float(guidance_rescale) if guidance_scale > 1.0 and guidance_rescale > 0.0 else 0.0
-
-
-def _step_kind(scheduler):
-    """The fused update a scheduler runs as: "euler" (EulerDiscreteScheduler), "ancestral"
-    (EulerAncestralDiscreteScheduler: the Euler update plus the noise term, ancestral_coeffs), "multistep"
-    (DDIMScheduler / DPMSolverMultistepScheduler, step_coeffs), "unipc" (UniPCMultistepScheduler, unipc_coeffs),
-    "heun" (HeunDiscreteScheduler, heun_coeffs), "lms" (LMSDiscreteScheduler, lms_coeffs) or "singlestep"
-    (DPMSolverSinglestepScheduler, singlestep_coeffs). Any other scheduler has no fused update here."""
-    if isinstance(scheduler, DPMSolverSinglestepScheduler):
-        return "singlestep"
-    if isinstance(scheduler, LMSDiscreteScheduler):
-        return "lms"
-    if isinstance(scheduler, HeunDiscreteScheduler):
-        return "heun"
-    if isinstance(scheduler, UniPCMultistepScheduler):
-        return "unipc"
-    if isinstance(scheduler, EulerAncestralDiscreteScheduler):
-        return "ancestral"
-    if isinstance(scheduler, EulerDiscreteScheduler):
-        return "euler"
-    if isinstance(scheduler, MULTISTEP_SCHEDULERS):
-        return "multistep"
-    raise TypeError(f"RegionDiffusionXL: unsupported scheduler {type(scheduler).__name__}; supported: "
-                    "EulerDiscreteScheduler, EulerAncestralDiscreteScheduler, DDIMScheduler, DPMSolverMultistepScheduler, "
-                    "UniPCMultistepScheduler, HeunDiscreteScheduler, LMSDiscreteScheduler, DPMSolverSinglestepScheduler "
-                    "(rtti_b200.schedulers)")
 
 
 class StableDiffusionXLPipelineOutput(dict):
@@ -319,85 +288,31 @@ class RegionDiffusionXL(LoraLoaderMixin):
     def _plain_loop(self, ctx, pooled, time_ids, latents, timesteps, guidance_scale, callback, callback_steps,
                     guidance_rescale=0.0, generator=None):
         """:879-914 — CFG batch [uncond, cond]; with capture armed the attention kernels accumulate the maps.
-        guidance_rescale rescales the CFG prediction inside the blend kernel (:903-905). A multistep scheduler: the UNet
-        sees the latents unscaled and the blend kernel takes the step_coeffs(i) update; UniPC likewise, with
-        unipc_coeffs(i) and three histories (ops.UniPCHistory). Euler Ancestral: the UNet input
-        is scaled as for Euler and the blend kernel adds s_up z, z [1, ...] drawn from `generator` after the UNet pass,
-        as the reference's step draws it (:908). Heun: iteration i scales the UNet input by sigma_i (sigma_at(i)) and
-        the blend kernel takes the heun_coeffs(i) update; a first stage keeps the latents it stepped and the stepped
-        prediction (two fp16 tensors, referenced until the second stage reads them: the blend writes fresh outputs and
-        nothing here writes in place). The callback follows the reference's rule (:874-877): iteration i calls it when
-        (i is the last iteration or (i + 1) % scheduler.order == 0) and i % callback_steps == 0 — every iteration
-        i % callback_steps == 0 for the order-1 schedulers, only second stages and the last iteration for Heun.
-        LMS: the UNet input is scaled as for Euler and the blend kernel takes the lms_coeffs(i) update on the fp16
-        predictions of the last three steps (blend outputs, referenced while they are in the history; nothing writes
-        them in place). DPM-Solver++(2S): the UNet sees the latents unscaled and the blend kernel takes the
-        singlestep_coeffs(i) update on one fp32 D buffer; a first step keeps the latents it stepped as the block's xs
-        (referenced until the second step reads them)."""
+        guidance_rescale rescales the CFG prediction inside the blend kernel (:903-905); the scheduler update runs in it
+        too (stepping.py), with Euler Ancestral's z [1, ...] drawn after the UNet pass, as the reference's step draws
+        it (:908). The callback follows the reference's rule (:874-877): iteration i calls it when (i is the last
+        iteration or (i + 1) % scheduler.order == 0) and i % callback_steps == 0 — every iteration
+        i % callback_steps == 0 for the order-1 schedulers, only second stages and the last iteration for Heun."""
         phi = _rescale_phi(guidance_scale, guidance_rescale)
         ctx2 = torch.cat([ctx[:1], ctx[-1:]])
         pooled2 = torch.cat([pooled[:1], pooled[-1:]])
         kv = CrossKVCache()
         ones = None
-        kind = _step_kind(self.scheduler)
-        multistep = kind == "multistep"
-        singlestep = kind == "singlestep"
-        d_hist = (torch.empty(latents.numel(), dtype=torch.float32, device=latents.device) if multistep or singlestep
-                  else None)
-        up_hist = ops.UniPCHistory(latents.numel(), latents.device) if kind == "unipc" else None
-        heun = kind == "heun"
-        xs = ds = None   # Heun: the latents and the prediction of the last first stage; 2S: xs, the block's latents
-        lms_hist = (None, None, None)   # LMS: the predictions of the last three steps, newest first
+        stepper = stepping.stepper(self.scheduler, latents.shape, latents.device, generator)
+        state = stepper.state()
         for i, t in enumerate(timesteps):
-            if multistep or singlestep or up_hist is not None:
-                x = latents.expand(2, -1, -1, -1)
-            else:
-                sigma = self.scheduler.sigma_at(i) if heun else self.scheduler.sigma(t)
-                x = (latents / math.sqrt(sigma * sigma + 1.0)).expand(2, -1, -1, -1)
+            norm = stepper.input_norm(i, t)
+            x = (latents if norm is None else latents / norm).expand(2, -1, -1, -1)
             ctrl = RegionControl(capture=self._capture, capture_row=1, kv_cache=kv)
             eps = self.unet(x, t, ctx2, {"text_embeds": pooled2, "time_ids": time_ids}, ctrl)["sample"]
             n = eps[0].numel()
             if ones is None:
                 ones = torch.ones(1, n, dtype=torch.float32, device=eps.device)
-            if multistep:
-                step = ops.MultistepStep(self.scheduler.step_coeffs(i), d_hist, d_hist)
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=latents.contiguous(), guidance_rescale=phi, step=step)
-            elif up_hist is not None:
-                step = ops.UniPCStep.of(self.scheduler.unipc_coeffs(i), up_hist)
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=latents.contiguous(), guidance_rescale=phi, step=step)
-                up_hist.rotate()
-            elif kind == "ancestral":
-                dt, s_up = self.scheduler.ancestral_coeffs(i)
-                z = self.scheduler.noise(tuple(latents.shape), generator, latents.device)
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=latents.contiguous(), guidance_rescale=phi,
-                                                  step=ops.AncestralStep(dt, s_up, z))
-            elif heun:
-                lat = latents.contiguous()
-                e16, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                    latents=lat, guidance_rescale=phi,
-                                                    step=ops.HeunStep(self.scheduler.heun_coeffs(i), xs, ds))
-                if self.scheduler.is_first_stage(i):
-                    xs, ds = lat, e16
-            elif kind == "lms":
-                e16, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                    latents=latents.contiguous(), guidance_rescale=phi,
-                                                    step=ops.LMSStep(self.scheduler.lms_coeffs(i), *lms_hist))
-                lms_hist = (e16,) + lms_hist[:2]
-            elif singlestep:
-                lat = latents.contiguous()
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=lat, guidance_rescale=phi,
-                                                  step=ops.SinglestepStep(self.scheduler.singlestep_coeffs(i), d_hist,
-                                                                          d_hist, xs))
-                if self.scheduler.is_first_step(i):
-                    xs = lat
-            else:
-                _, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
-                                                  latents=latents.contiguous(), dt_sigma=self.scheduler.dt(t),
-                                                  guidance_rescale=phi)
+            stepper.begin(i, t, 1)
+            lat = latents.contiguous()
+            e16, latents = ops.region_blend_cfg(eps[0:1].contiguous(), [eps[1:2].contiguous()], ones, guidance_scale,
+                                                latents=lat, guidance_rescale=phi, step=stepper.step(state))
+            state = stepper.advance(state, lat, e16)
             if callback is not None and self._calls_back(i, len(timesteps), callback_steps):
                 callback(i, t, latents)
         return latents
@@ -455,29 +370,10 @@ class RegionDiffusionXL(LoraLoaderMixin):
         st.kv_caches = {}
         st.graphs = {}
         st.noise_pred = None
-        # multistep schedulers: one fp32 history of the x0 prediction per trajectory (main, reference)
-        kind = _step_kind(self.scheduler)
-        st.multistep, st.ancestral, st.unipc = kind == "multistep", kind == "ancestral", kind == "unipc"
-        st.generator = generator
-        n = latents.numel()
-        st.d_hist = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep else None
-        st.d_hist_ref = torch.empty(n, dtype=torch.float32, device=dev) if st.multistep and inject else None
-        # UniPC: one state of three fp32 buffers per trajectory
-        st.up_hist = ops.UniPCHistory(n, dev) if st.unipc else None
-        st.up_hist_ref = ops.UniPCHistory(n, dev) if st.unipc and inject else None
-        # Heun: (latents, prediction) of the last first stage per trajectory, fp16, referenced until the second stage
-        st.heun = kind == "heun"
-        st.heun_main = st.heun_ref = (None, None)
-        # LMS: the fp16 predictions of the last three steps per trajectory, newest first
-        st.lms = kind == "lms"
-        st.lms_main = st.lms_ref = (None, None, None)
-        # DPM-Solver++(2S): the D buffers of the multistep schedulers, and the fp16 latents that entered the current
-        # block's first step per trajectory (referenced until its second step)
-        st.singlestep = kind == "singlestep"
-        if st.singlestep:
-            st.d_hist = torch.empty(n, dtype=torch.float32, device=dev)
-            st.d_hist_ref = torch.empty(n, dtype=torch.float32, device=dev) if inject else None
-        st.ss_xs = st.ss_xs_ref = None
+        # the fused scheduler update and its state per trajectory (main, reference)
+        st.stepper = stepping.stepper(self.scheduler, latents.shape, dev, generator)
+        st.main = st.stepper.state()
+        st.ref = st.stepper.state() if inject else None
         return st
 
     def _unet_pass(self, st, x, t, local, feat_inject_step):
@@ -572,11 +468,7 @@ class RegionDiffusionXL(LoraLoaderMixin):
         passes, kind, plan, N = st.passes, st.kind, st.plan, st.N
         feat_inject_step = bool(float(t) > (1 - st.inject_selfattn) * 1000)            # :782
         background_inject_step = i < st.inject_background * st.n_t                      # :783
-        if st.multistep or st.unipc or st.singlestep:   # scale_model_input is the identity
-            scale = None
-        else:
-            sigma = self.scheduler.sigma_at(i) if st.heun else self.scheduler.sigma(t)
-            scale = 1.0 / math.sqrt(sigma * sigma + 1.0)                                # :784
+        norm = st.stepper.input_norm(i, t)                                               # :784
         if feat_inject_step and st.inject:
             self._remote_qk(st, st.latents)   # collective on first use: every rank of the group, also those without passes
         local = plan.local_passes(feat_inject_step)
@@ -586,8 +478,8 @@ class RegionDiffusionXL(LoraLoaderMixin):
             ev[0].record()
         if local:
             x = torch.cat([(st.latents_ref if passes[p]["ref"] else st.latents) for p in local])
-            if scale is not None:
-                x = x * scale
+            if norm is not None:
+                x = x * (1.0 / norm)
             eps_local = self._unet_pass(st, x, t, local, feat_inject_step)
         else:   # more ranks than passes on this step: this rank only takes part in the exchange
             eps_local = st.latents.new_empty((0,) + tuple(st.latents.shape[1:]))
@@ -598,66 +490,11 @@ class RegionDiffusionXL(LoraLoaderMixin):
         if pe is not None:
             ev[1].record()
         step_ref = st.inject and (st.inject_selfattn > 0 or background_inject_step)                       # :830-841
-        if st.multistep:
-            c = self.scheduler.step_coeffs(i)
-            dt = 0.0
-            step = ops.MultistepStep(c, st.d_hist, st.d_hist, st.d_hist_ref, st.d_hist_ref)
-            step_main = ops.MultistepStep(c, st.d_hist, st.d_hist)
-            step_refl = ops.MultistepStep(c, st.d_hist_ref, st.d_hist_ref)
-        elif st.unipc:
-            c = self.scheduler.unipc_coeffs(i)
-            dt = 0.0
-            step = ops.UniPCStep.of(c, st.up_hist, st.up_hist_ref if step_ref else None)
-            step_main = ops.UniPCStep.of(c, st.up_hist)
-            step_refl = ops.UniPCStep.of(c, st.up_hist_ref) if step_ref else None
-        elif st.ancestral:
-            # the reference draws z in its scheduler step (:837-846): one [2, ...] draw when it steps both trajectories
-            # as one batch (main first), [1, ...] otherwise; on CUDA one [2, n] draw differs from two [1, n] draws
-            dt = 0.0
-            a_dt, s_up = self.scheduler.ancestral_coeffs(i)
-            z = self.scheduler.noise((2 if step_ref else 1,) + tuple(st.latents.shape[1:]), st.generator, self.device)
-            z_ref = z[1:2] if step_ref else None
-            step = ops.AncestralStep(a_dt, s_up, z[0:1], z_ref)
-            step_main, step_refl = ops.AncestralStep(a_dt, s_up, z[0:1]), ops.AncestralStep(a_dt, s_up, z_ref)
-        elif st.heun:
-            # each trajectory steps from its own saved state; a first stage saves the latents it steps and their
-            # prediction (on the fused exchange the reference trajectory's is written into eps_ref)
-            dt = 0.0
-            c = self.scheduler.heun_coeffs(i)
-            first = self.scheduler.is_first_stage(i)
-            st.latents = lat_in = st.latents.contiguous()
-            if step_ref:
-                st.latents_ref = ref_in = st.latents_ref.contiguous()
-            xs_ref, ds_ref = st.heun_ref if step_ref else (None, None)
-            fused = plan.world > 1 and self.fused_exchange
-            eps_ref = torch.empty_like(ref_in) if first and step_ref and fused else None
-            step = ops.HeunStep(c, *st.heun_main, xs_ref, ds_ref, eps_ref)
-            step_main, step_refl = ops.HeunStep(c, *st.heun_main), ops.HeunStep(c, xs_ref, ds_ref)
-        elif st.lms:
-            # each trajectory steps on its own history (on the fused exchange the reference trajectory's prediction is
-            # written into eps_ref)
-            dt = 0.0
-            c = self.scheduler.lms_coeffs(i)
-            hist_ref = st.lms_ref if step_ref else (None, None, None)
-            fused = plan.world > 1 and self.fused_exchange
-            eps_ref = torch.empty_like(st.latents_ref) if step_ref and fused else None
-            step = ops.LMSStep(c, *st.lms_main, *hist_ref, eps_ref)
-            step_main, step_refl = ops.LMSStep(c, *st.lms_main), ops.LMSStep(c, *hist_ref)
-        elif st.singlestep:
-            # each trajectory steps on its own D buffer; a first step keeps the latents it steps as its block's xs
-            dt = 0.0
-            c = self.scheduler.singlestep_coeffs(i)
-            first = self.scheduler.is_first_step(i)
-            st.latents = lat_in = st.latents.contiguous()
-            if step_ref:
-                st.latents_ref = ref_in = st.latents_ref.contiguous()
-            xs_ref = st.ss_xs_ref if step_ref else None
-            step = ops.SinglestepStep(c, st.d_hist, st.d_hist, st.ss_xs, st.d_hist_ref, st.d_hist_ref, xs_ref)
-            step_main = ops.SinglestepStep(c, st.d_hist, st.d_hist, st.ss_xs)
-            step_refl = ops.SinglestepStep(c, st.d_hist_ref, st.d_hist_ref, xs_ref)
-        else:
-            dt = self.scheduler.dt(t)
-            step = step_main = step_refl = None
+        stepper = st.stepper
+        stepper.begin(i, t, 2 if step_ref else 1)
+        st.latents = lat = st.latents.contiguous()
+        if step_ref:
+            st.latents_ref = lat_ref = st.latents_ref.contiguous()
         ex = None
         if plan.world > 1 and self.fused_exchange:
             xkey = (tuple(p["kind"] for p in passes), st.latents[0].numel())
@@ -670,46 +507,31 @@ class RegionDiffusionXL(LoraLoaderMixin):
                     self.fused_exchange = False
             ex = self._exchanges.get(xkey)
         if ex is not None:
-            # fused all-gather + blend + CFG + scheduler update over NVLink peer memory (csrc/gather_blend.cu)
+            # fused all-gather + blend + CFG + scheduler update over NVLink peer memory (csrc/gather_blend.cu); the
+            # reference trajectory's stepped prediction is written into eps_ref where its state keeps it
             _, owner = plan._plan(feat_inject_step)
             sid = ex.publish(eps_local, local, owner)
+            eps_ref = torch.empty_like(lat_ref) if step_ref and stepper.writes_eps_ref() else None
             st.noise_pred, st.latents, ref_out = ops.gather_blend_step(
-                ex.slot_ptrs, ex.flag_ptrs, ex.rank, ex.slot_owner(owner), N, st.masks, st.guidance_scale,
-                st.latents.contiguous(), st.latents_ref.contiguous() if step_ref else None, dt, sid,
-                guidance_rescale=st.guidance_rescale, step=step)
+                ex.slot_ptrs, ex.flag_ptrs, ex.rank, ex.slot_owner(owner), N, st.masks, st.guidance_scale, lat,
+                lat_ref if step_ref else None, 0.0, sid, guidance_rescale=st.guidance_rescale,
+                step=stepper.step_pair(st.main, st.ref, step_ref, eps_ref))
             if step_ref:
                 st.latents_ref = ref_out
         else:
             eps = plan.gather(eps_local, local, feat_inject_step)   # NCCL all-gather; identity on one GPU
             one = lambda name: eps[kind[name]:kind[name] + 1].contiguous()
             regions = [one(f"E{j}") for j in range(N - 1)] + [one("B")]
-            st.noise_pred, st.latents = ops.region_blend_cfg(one("A"), regions, st.masks, st.guidance_scale,
-                                                              latents=st.latents.contiguous(), dt_sigma=dt,
+            st.noise_pred, st.latents = ops.region_blend_cfg(one("A"), regions, st.masks, st.guidance_scale, latents=lat,
                                                               guidance_rescale=st.guidance_rescale,
-                                                              step=step_main)  # :810-830
+                                                              step=stepper.step(st.main))  # :810-830
             if step_ref:
-                eps_cd, st.latents_ref = ops.region_blend_cfg(one("C"), [one("D")], st.ones, st.guidance_scale,
-                                                              latents=st.latents_ref.contiguous(), dt_sigma=dt,
-                                                              guidance_rescale=st.guidance_rescale,
-                                                              step=step_refl)
-                if st.heun or st.lms:
-                    eps_ref = eps_cd
-        if st.unipc:   # this step's x0 prediction becomes m1 of the next step
-            st.up_hist.rotate()
-            if step_ref:
-                st.up_hist_ref.rotate()
-        if st.heun and first:
-            st.heun_main = (lat_in, st.noise_pred)
-            if step_ref:
-                st.heun_ref = (ref_in, eps_ref)
-        if st.singlestep and first:
-            st.ss_xs = lat_in
-            if step_ref:
-                st.ss_xs_ref = ref_in
-        if st.lms:
-            st.lms_main = (st.noise_pred,) + st.lms_main[:2]
-            if step_ref:
-                st.lms_ref = (eps_ref,) + st.lms_ref[:2]
+                eps_ref, st.latents_ref = ops.region_blend_cfg(one("C"), [one("D")], st.ones, st.guidance_scale,
+                                                               latents=lat_ref, guidance_rescale=st.guidance_rescale,
+                                                               step=stepper.step(st.ref, 1))
+        st.main = stepper.advance(st.main, lat, st.noise_pred)
+        if step_ref:
+            st.ref = stepper.advance(st.ref, lat_ref, eps_ref)
         if pe is not None:
             ev[2].record()
         if st.use_guidance and float(t) < st.tfd["guidance_start_step"]:                                  # :849

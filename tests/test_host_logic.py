@@ -25,6 +25,43 @@ def test_library_exports_every_declared_symbol():
     assert lib.rtti_color_loss_workspace_elems(2, 1024 * 1024) > 0
 
 
+_C_ABI = {"int": "int32", "int32_t": "int32", "long long": "int64", "int64_t": "int64", "unsigned": "uint32",
+          "unsigned int": "uint32", "uint32_t": "uint32", "unsigned long long": "uint64", "uint64_t": "uint64",
+          "size_t": "uint64", "float": "float", "double": "double"}
+
+
+def _c_abi(decl):
+    """ABI class of a C type, with or without a parameter name."""
+    if "*" in decl:
+        return "pointer"
+    words = [w for w in decl.split() if w != "const"]
+    base = " ".join(words[:-1]) if len(words) > 1 and " ".join(words) not in _C_ABI else " ".join(words)
+    return _C_ABI[base]
+
+
+def _ctypes_abi(ty):
+    if ty is ctypes.c_void_p or issubclass(ty, ctypes._Pointer):
+        return "pointer"
+    if ty in (ctypes.c_float, ctypes.c_double):
+        return ty.__name__[2:]
+    return ("int" if ty(-1).value < 0 else "uint") + str(8 * ctypes.sizeof(ty))
+
+
+def test_binding_argument_types_match_the_header():
+    """Every prototype of the header against _lib.SIGNATURES, parameter by parameter: a miscounted or misplaced float
+    or pointer would otherwise only show as wrong arguments on the GPU."""
+    from rtti_b200 import _lib
+    header = open(os.path.join(ROOT, "include", "rtti_b200.h")).read()
+    header = re.sub(r"/\*.*?\*/|//[^\n]*|^\s*#[^\n]*", "", header, flags=re.S | re.M)
+    protos = re.findall(r"([A-Za-z_][\w\s]*?)\s+(rtti_\w+)\s*\(([^)]*)\)\s*;", header)
+    assert len(protos) == len(_lib.SIGNATURES)
+    for ret, name, params in protos:
+        params = [] if params.strip() in ("", "void") else [p.strip() for p in params.split(",")]
+        restype, argtypes = _lib.SIGNATURES[name]
+        assert _c_abi(ret) == _ctypes_abi(restype), name
+        assert [_c_abi(p) for p in params] == [_ctypes_abi(t) for t in argtypes], name
+
+
 def test_tensor_core_kernels_fit_the_launch_time_register_check():
     """The hardware verifies a launch's register demand with the CTA's warp count rounded up to the 4 SM sub-partitions
     (cuda_occupancy.h, "Hardware check"): a 9-warp CTA is checked as 12 warps. A kernel over the limit compiles and
