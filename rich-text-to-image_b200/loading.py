@@ -10,6 +10,7 @@ import os
 
 import torch
 
+from .textual_inversion import expand_prompt
 from .unet import UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -78,6 +79,7 @@ class ClipTextEncoders:
                 os.path.join(root, "text_encoder_2"), torch_dtype=torch.float16).to(device)
 
     def _ids(self, tok, prompts, device):
+        prompts = [expand_prompt(tok, p) for p in prompts]   # multi-vector textual-inversion tokens (textual_inversion.py)
         return tok(prompts, padding="max_length", max_length=tok.model_max_length, truncation=True,
                    return_tensors="pt").input_ids.to(device)
 

@@ -21,6 +21,7 @@ from . import ops, region_parallel, stepping, vae_guidance
 from .attention_utils import CrossAttentionLayers, SelfAttentionLayers
 from .lora import LoraLoaderMixin
 from .schedulers import PNDMScheduler
+from .textual_inversion import TextualInversionLoaderMixin
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -29,7 +30,7 @@ from .vae import AutoencoderKLDecoder, VAEConfig
 _FUSED = ("multistep", "unipc", "singlestep")
 
 
-class RegionDiffusion(LoraLoaderMixin):
+class RegionDiffusion(LoraLoaderMixin, TextualInversionLoaderMixin):
     def __init__(self, device="cuda", unet=None, vae=None, text_encoder=None, load_path="runwayml/stable-diffusion-v1-5"):
         self.device = torch.device(device)
         torch.backends.cudnn.benchmark = True   # static shapes: let cuDNN pick its fastest conv algorithm once
@@ -60,6 +61,10 @@ class RegionDiffusion(LoraLoaderMixin):
 
     def _lora_components(self):
         return self.unet, (() if self.text_encoder is None else (self.text_encoder.text_encoder,))
+
+    def _textual_inversion_components(self):
+        te = self.text_encoder
+        return [] if te is None else [(te.tokenizer, te.text_encoder)]
 
     # ------------------------------------------------------------------ capture API (:397-450)
     def register_tokenmap_hooks(self):

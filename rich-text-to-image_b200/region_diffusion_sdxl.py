@@ -25,6 +25,7 @@ from .attention_utils import CrossAttentionLayers_XL
 from .lora import LoraLoaderMixin
 from .schedulers import DDIMScheduler, EulerDiscreteScheduler
 from .stepping import _step_kind  # noqa: F401  (re-exported)
+from .textual_inversion import TextualInversionLoaderMixin
 from .unet import CrossKVCache, RegionControl, TokenMapAccumulator, UNet2DConditionModel, UNetConfig
 from .vae import AutoencoderKLDecoder, VAEConfig
 
@@ -40,7 +41,7 @@ class StableDiffusionXLPipelineOutput(dict):
         self.images = images
 
 
-class RegionDiffusionXL(LoraLoaderMixin):
+class RegionDiffusionXL(LoraLoaderMixin, TextualInversionLoaderMixin):
     def __init__(self, load_path: str = "stabilityai/stable-diffusion-xl-base-1.0", device: str = "cuda",
                  force_zeros_for_empty_prompt: bool = True, unet=None, vae=None, scheduler=None,
                  text_encoders=None):
@@ -113,6 +114,10 @@ class RegionDiffusionXL(LoraLoaderMixin):
     def _lora_components(self):
         te = self.text_encoders
         return self.unet, (() if te is None else (te.text_encoder, te.text_encoder_2))
+
+    def _textual_inversion_components(self):
+        te = self.text_encoders
+        return [] if te is None else [(te.tokenizer, te.text_encoder), (te.tokenizer_2, te.text_encoder_2)]
 
     # ------------------------------------------------------------------ helpers
     def encode_prompt(self, prompt, negative_prompt):

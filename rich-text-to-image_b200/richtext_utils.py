@@ -12,6 +12,8 @@ import random
 import numpy as np
 import torch
 
+from .textual_inversion import tokenize
+
 COLORS = {
     "brown": (165, 42, 42), "red": (255, 0, 0), "pink": (253, 108, 158), "orange": (255, 165, 0),
     "yellow": (255, 255, 0), "purple": (128, 0, 128), "green": (0, 128, 0), "blue": (0, 0, 255),
@@ -117,8 +119,9 @@ def parse_json(json_str, device=None):
 
 
 def _positions(tokenizer, base_tokens, text):
-    """1-based index in the base prompt of the FIRST occurrence of each BPE token of `text`."""
-    return [base_tokens.index(tok) + 1 for tok in tokenizer._tokenize(text)]
+    """1-based index in the base prompt of the FIRST occurrence of each BPE token of `text`. A textual-inversion
+    token of n vectors is n tokens here, as in the encoded prompt."""
+    return [base_tokens.index(tok) + 1 for tok in tokenize(tokenizer, text)]
 
 
 def _with_rest(groups, n_tokens):
@@ -132,7 +135,7 @@ def get_region_diffusion_input(model, base_text_prompt, style_text_prompts, foot
     """Algorithm 1 of the paper: region prompts [styles..., footnotes..., colours..., base] and the
     1-based token ids each region is anchored on (last entry: all remaining tokens)."""
     tok = model.tokenizer
-    base_tokens = tok._tokenize(base_text_prompt)
+    base_tokens = tokenize(tok, base_text_prompt)
     prompts, ids = [], []
     for p in style_text_prompts:
         prompts.append(p)

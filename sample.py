@@ -9,7 +9,9 @@ DPM-Solver++(2M) is the usual choice at about 20 --sample_steps, UniPC the sampl
 DPM-Solver++(2S), the singlestep variant; euler_a, Euler Ancestral, heun, Heun's
 second-order method, which evaluates the UNet 2N - 1 times for N --sample_steps, and lms, k-LMS, are for SDXL / AnimeXL
 only), --lora_path (a LOCAL LoRA .safetensors file, kohya or diffusers format, merged into the UNet and text-encoder
-weights) with --lora_scale (default 1.0).
+weights) with --lora_scale (default 1.0), and --textual_inversion PATH[:TOKEN] (repeatable; a LOCAL textual-inversion
+embedding, diffusers, A1111 or SDXL format, added to the tokenizers after the LoRA; TOKEN defaults to the token the file
+names).
 """
 import argparse
 import json
@@ -59,6 +61,11 @@ def main(args, param):
                            "heun": HeunDiscreteScheduler, "lms": LMSDiscreteScheduler}[args.scheduler]()
     if args.lora_path is not None:
         model.load_lora_weights(args.lora_path, scale=args.lora_scale)
+    for spec in args.textual_inversion:
+        path, sep, token = spec.rpartition(":")
+        if not (sep and os.path.exists(path)):   # no ":TOKEN" suffix (or a ':' inside the path)
+            path, token = spec, None
+        model.load_textual_inversion(path, token=token or None)
 
     (base_prompt, style_prompts, footnote_prompts, footnote_targets, color_prompts, color_names, color_rgbs,
      sizes, use_grad_guidance) = parse_json(param["text_input"])
@@ -131,6 +138,7 @@ if __name__ == "__main__":
                    choices=["default", "ddim", "dpmpp_2m", "dpmpp_2s", "euler_a", "unipc", "heun", "lms"])
     p.add_argument("--lora_path", type=str, default=None)
     p.add_argument("--lora_scale", type=float, default=1.0)
+    p.add_argument("--textual_inversion", action="append", default=[], metavar="PATH[:TOKEN]")
     a = p.parse_args()
     res = 512 if a.model == "SD" else 1024
     main(a, {"text_input": json.loads(a.rich_text_json), "height": a.height or res, "width": a.width or res,
